@@ -673,3 +673,8 @@ def fr_dot_device(worker, d_a, d_b, n):
     out = np.zeros(4, np.uint64)
     _check(load_library().bb_diag_fr_dot(worker._h, d_a, d_b, C.c_size_t(n), _ptr(out)))
     return out
+
+
+# groth16 verification (groth16/src/verifier.rs, verifier/batch.rs)
+from .verifier import (BatchVerifier, InvalidProof, InvalidVerifyingKey, PreparedVerifyingKey,  # noqa: E402
+                       VerificationError, prepare_verifying_key, verify_proof)

@@ -1,0 +1,167 @@
+#!/usr/bin/env python
+"""bench_verify.py -- Groth16 batch verification throughput on H100 (batch::Verifier::verify,
+groth16/src/verifier/batch.rs:100-173, through bb_groth16_verify_batch).
+
+    python bench_verify.py --steps K --warmup W [--log-size 12] [--inputs 7] [--dump-outputs DIR]
+
+A step verifies one batch of 2^log-size synthetic proofs with --inputs public inputs each.  The proofs come from
+bb_synth_proof_batch (trapdoor scalars, fixed-base multiplications on the device) before the timed region, and the
+random z_i from a seeded generator, so every run sees the same batch.  `value` is proofs/s with the batch resident in
+HBM, `e2e` the same batch from pinned host buffers.  Outside the timed regions the script asserts that the batch is
+accepted and that the same batch with C_0 replaced by C_1 is rejected.  The line carries the per-stage device
+milliseconds (CUDA events of the library's profile mode) and the Fp-multiplication rate of the Miller loops.
+
+--dump-outputs DIR writes the two verdicts and the G_T value of the rejected batch (deterministic under the seeded z)
+as float64 .npy files, the format of bench.py --dump-outputs.  Prints one JSON line on stdout; writes nothing else.
+"""
+import argparse
+import importlib.util
+import os
+import random
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, ROOT)
+
+_spec = importlib.util.spec_from_file_location("bench", os.path.join(ROOT, "bench.py"))
+bench = importlib.util.module_from_spec(_spec)             # the clock sampler, emit / log and the dump format of bench.py
+_spec.loader.exec_module(bench)
+
+FR_MODULUS = bench.FR_MODULUS
+DEFAULT_LOG = 12        # 4096 proofs: about the Sapling spend proofs of one full 2 MB Zcash block (384-byte spend descriptions)
+DEFAULT_INPUTS = 7      # public inputs of a Sapling spend proof (rk, cv, anchor, nullifier as Fr elements)
+FP_MUL_PEAK = 27.3      # G Fp-mul/s: tools/ubench.cu k_fmul<Fp>, best launch shape, H100 SXM 80 GB at a 700 W power limit
+
+
+def parse():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--gpus", type=int, default=1, choices=[1], help="one device (multi-GPU verification is not implemented)")
+    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--log-size", type=int, default=DEFAULT_LOG, help="log2 of the proofs per batch")
+    ap.add_argument("--inputs", type=int, default=DEFAULT_INPUTS, help="public inputs per proof")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the verdicts and the rejected batch's G_T value as DIR/<name>.npy")
+    return ap.parse_args()
+
+
+def miller_fp_muls_per_pair():
+    """Fp multiplications of one pair's Miller loop in csrc/tower.cuh, from its step counts: an Fp2 product costs 3 Fp
+    products, an Fp2 squaring or an Fp2 x Fp product 2."""
+    fp12_sqr = 2 * 6 * 3                                    # two Fp6 products of 6 Fp2 products
+    mul_line = 15 * 3                                       # fp12_mul_line: 15 Fp2 products
+    dbl = 5 * 2 + 3 * 2 + 4 * 3                             # miller_dbl_step: 5 Fp2 squarings, 3 Fp2 x Fp, 4 Fp2 products
+    add = 11 * 3 + 3 * 2 + 2 * 2                            # miller_add_step: 11 Fp2 products, 3 Fp2 x Fp, 2 Fp2 squarings
+    return 63 * (fp12_sqr + dbl + mul_line) + 5 * (add + mul_line)
+
+
+def run(args):
+    import torch
+
+    import bellman_b200 as bb
+    from bellman_b200 import verifier as V
+    log_n, L = args.log_size, args.inputs
+    if L < 0:
+        raise SystemExit("--inputs must be >= 0")
+    n = 1 << log_n
+    worker = bb.Worker(0)
+    bench.log(f"generating {n} synthetic proofs with {L} public inputs on the device")
+    d = {"a": worker.device_alloc(n * 96), "b": worker.device_alloc(n * 192), "c": worker.device_alloc(n * 96),
+         "x": worker.device_alloc(max(1, n * L) * 32)}
+    vk = V.synth_proof_batch(worker, 51, n, L, d["a"], d["b"], d["c"], d["x"])
+    pvk = bb.prepare_verifying_key(worker, vk)
+
+    keep, host = [], {}                                     # the same batch in page-locked host memory (e2e leg)
+    for key, shape in (("a", (n, 12)), ("b", (n, 24)), ("c", (n, 12)), ("x", (n, L, 4))):
+        t = torch.zeros(shape, dtype=torch.int64).pin_memory()
+        keep.append(t)
+        arr = t.numpy().view(np.uint64)
+        if arr.size:
+            worker.download(d[key], arr)
+        host[key] = arr
+    rng = random.Random(52)
+    z = [rng.randrange(1, FR_MODULUS) for _ in range(n)]
+
+    def step_value():
+        V.verify_batch_arrays(pvk, d["a"], d["b"], d["c"], d["x"], z=z, on_device=True, n=n, n_inputs=L)
+
+    def step_e2e():
+        V.verify_batch_arrays(pvk, host["a"], host["b"], host["c"], host["x"], z=z, n_inputs=L)
+
+    def timed(step):
+        for _ in range(args.warmup):
+            step()
+        worker.synchronize()
+        worker.profile_reset()
+        l0 = worker.kernel_launches
+        h0, _ = worker.bytes_copied()
+        t0 = time.perf_counter()
+        for _ in range(args.steps):
+            step()
+        worker.synchronize()
+        dt = time.perf_counter() - t0
+        h1, _ = worker.bytes_copied()
+        return dt, worker.kernel_launches - l0, (h1 - h0) / args.steps
+
+    bench.log("timed region: batch resident in HBM")
+    sampler = bench.ClockSampler(0)
+    sampler.start()
+    worker.set_option("profile", 1)
+    dt_val, launches, _ = timed(step_value)
+    clocks = sampler.stop()
+    stage = lambda *names: sum(worker.profile_read(nm)[0] for nm in names) / args.steps
+    stages = {"accumulators": stage("verify.accumulators"), "scalar_mul": stage("verify.scalar_mul"),
+              "msms": stage("msm_total_g1"), "msm_wait": stage("verify.msm_wait"),
+              "miller": stage("verify.miller", "verify.miller_tail"), "product": stage("verify.product"),
+              "final_exp": stage("verify.final_exp")}
+    worker.set_option("profile", 0)
+    bench.log(f"value leg: {1e3 * dt_val / args.steps:.2f} ms/step; timed region: pinned host buffers (e2e)")
+    dt_e2e, _, h2d = timed(step_e2e)
+    # outside the timed regions: the timed batch is accepted, and the same batch with C_0 replaced by C_1 is rejected
+    ok, _ = V.verify_batch_arrays(pvk, d["a"], d["b"], d["c"], d["x"], z=z, on_device=True, n=n, n_inputs=L, gt=True)
+    c_bad = host["c"].copy()
+    c_bad[0] = host["c"][1 % n]
+    ok_bad, gt_bad = V.verify_batch_arrays(pvk, host["a"], host["b"], c_bad, host["x"], z=z, n_inputs=L, gt=True)
+    checks = {"timed_batch": "accepted" if ok else "REJECTED", "one_c_replaced": "rejected" if not ok_bad else "ACCEPTED"}
+    per_pair = miller_fp_muls_per_pair()
+    miller_ms = stages["miller"]
+    line = {"metric": "groth16_batch_verify_proofs_per_sec", "value": n * args.steps / dt_val, "unit": "proofs/s", "n_gpus": 1,
+            "steps": args.steps, "warmup": args.warmup, "ms_per_step": 1e3 * dt_val / args.steps, "higher_is_better": True,
+            "scaling": "strong", "vs_baseline": None, "dtype": "u32 limbs (381-bit Fp / 255-bit Fr Montgomery integers)", "data": "synthetic",
+            "config": {"workload": f"groth16-batch-verify-2^{log_n}", "proofs": n, "inputs_per_proof": L, "pairs": n + 3,
+                       "proofs_source": "bb_synth_proof_batch: [a]G1, [b]G2, [c]G1 from trapdoor scalars, made on the device before the timed region",
+                       "z": "seeded (random.Random(52)), canonical, uploaded each step",
+                       "timing": "host wall clock over K steps bracketed by device synchronize; stages by CUDA events on the main stream "
+                                 "(msms: the two MSM jobs on their own streams, summed)",
+                       "checks": checks},
+            "e2e": {"value": n * args.steps / dt_e2e, "unit": "proofs/s", "h2d_bytes_per_step": int(h2d), "ms_per_step": 1e3 * dt_e2e / args.steps},
+            "gpu_launches": int(launches), "clocks": clocks,
+            "stages_ms_per_step": {k: round(v, 3) for k, v in stages.items()},
+            "fp_mul": {"per_pair_miller": per_pair, "unit": "G Fp-mul/s",
+                       "miller_rate": (per_pair * (n + 3) / (miller_ms * 1e-3) / 1e9) if miller_ms > 0 else None,
+                       "peak": FP_MUL_PEAK, "peak_source": "tools/ubench.cu k_fmul<Fp>, best launch shape, on an H100 SXM (80 GB HBM3, 700 W power limit)",
+                       "model": "miller_fp_muls_per_pair(): 63 doubling and 5 addition steps of csrc/tower.cuh counted in Fp products"},
+            "cpu_baseline": None,
+            "cpu_baseline_reason": "oracle-1 has no CPU pairing; the Python pairing of oracle-0 is a correctness reference, not a timed baseline"}
+    bench.dump_outputs(args.dump_outputs, {"verdicts": np.array([int(ok), int(ok_bad)], np.uint32), "gt_tampered": gt_bad})
+    bench.emit(line)
+    assert ok and not ok_bad, checks
+    pvk.free()
+    for p in d.values():
+        worker.device_free(p)
+    worker.close()
+
+
+def main():
+    args = parse()
+    # stdout carries exactly ONE JSON line: whatever libraries print goes to stderr until the result is ready
+    sys.stdout.flush()
+    bench._REAL_STDOUT = os.dup(1)
+    os.dup2(2, 1)
+    run(args)
+
+
+if __name__ == "__main__":
+    main()

@@ -40,6 +40,9 @@ typedef enum bb_status {
     BB_ERR_UNEXPECTED_IDENTITY = 2,         /* multiexp.rs:63-65, prover.rs:320-324 */
     BB_ERR_IO_UNEXPECTED_EOF = 3,           /* multiexp.rs:55-61,74-80 */
     BB_ERR_DENSITY_MISMATCH = 5,            /* the assert! at multiexp.rs:324-329 (a panic upstream) */
+    /* VerificationError (src/lib.rs:353-358) */
+    BB_ERR_INVALID_VERIFYING_KEY = 6,       /* inputs.len() + 1 != ic.len(): verifier.rs:28-30, batch.rs:105-111 */
+    BB_ERR_INVALID_PROOF = 7,               /* the pairing equation does not hold */
     /* back-end errors */
     BB_ERR_ARG = 16,
     BB_ERR_CUDA = 17,
@@ -263,6 +266,38 @@ int bb_groth16_finalize_with(const bb_crs* crs, const uint8_t* partials, size_t 
  * b_g1_inputs, b_g1_aux, b_g2_inputs, b_g2_aux, h, l (:339-354). */
 int bb_groth16_prove(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w,
                      const uint8_t r[32], const uint8_t s[32], uint8_t proof[192]);
+
+/* ---- verification: groth16/src/verifier.rs and groth16/src/verifier/batch.rs ------------------
+ * Points are taken as valid curve and subgroup elements, as the reference's Proof / VerifyingKey types guarantee
+ * through read(); bb_points_validate applies those checks.  The identity is allowed anywhere: a pair with an identity
+ * on either side contributes one to the Miller product, as in bls12_381's multi_miller_loop. */
+/* PreparedVerifyingKey (groth16/src/lib.rs:400-409, verifier.rs:11-21): the verifying key resident on the device */
+typedef struct bb_vk_desc {
+    const void* alpha_g1;                                             /* 96 B */
+    const void* beta_g2; const void* gamma_g2; const void* delta_g2;  /* 192 B each */
+    const void* ic; size_t ic_len;                                    /* 96 B each */
+} bb_vk_desc;
+typedef struct bb_vk bb_vk;
+int bb_vk_prepare(bb_ctx* ctx, const bb_vk_desc* desc, bb_vk** out);
+void bb_vk_destroy(bb_vk* vk);
+
+/* batch::Item x n (batch.rs:40-43): proofs as affine points in the format above (a, c: G1; b: G2), inputs n x n_inputs
+ * Fr (Montgomery, row-major).  on_device != 0: a, b, c and inputs are device pointers. */
+typedef struct bb_proof_batch {
+    const void* a; const void* b; const void* c; size_t n;
+    const void* inputs; size_t n_inputs;
+    int on_device;
+} bb_proof_batch;
+
+/* verify_proof (verifier.rs:23-58): host buffers, one proof.  BB_OK = valid, BB_ERR_INVALID_PROOF = the equation fails,
+ * BB_ERR_INVALID_VERIFYING_KEY = n_inputs + 1 != ic_len.  Computed as the batch of one with z = 1. */
+int bb_groth16_verify(bb_ctx* ctx, const bb_vk* vk, const void* a, const void* b, const void* c,
+                      const void* inputs, size_t n_inputs);
+/* batch::Verifier::verify (batch.rs:100-173): one multi-Miller loop over the n + 3 pairs
+ * (z_i A_i, -B_i), (sum z_i C_i, delta), (Psi, gamma), ([sum z_i] alpha, beta) and one final exponentiation.
+ * z: n canonical 32-byte scalars in [1, r) (zero or >= r: BB_ERR_ARG), or NULL = drawn from the operating system
+ * (getrandom, zeros redrawn).  The key check comes first, before any device work.  An empty batch is accepted. */
+int bb_groth16_verify_batch(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* batch, const void* z);
 
 /* ---- tuning per key ------------------------------------------------------------------------
  * The MSM has several forms with identical results (per-window bucket sets; one bucket set over resident window

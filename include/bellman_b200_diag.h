@@ -42,6 +42,25 @@ int bb_selftest_bucket_reduce(bb_ctx* ctx, const void* affine_pts, uint32_t D, u
  * (the naive == fast property of src/multiexp.rs:334-378 at any size). */
 int bb_diag_fr_dot(bb_ctx* ctx, const void* d_a, const void* d_b, size_t n, void* out_fr);
 
+/* ---- pairing (verify.cu) ---------------------------------------------------------------------- */
+/* prod_i e(P_i, Q_i) after the final exponentiation, P_i / Q_i affine host arrays (identity allowed); gt_out: 12 canonical
+ * Fp (6 x u64 each) in tower order c0.c0.c0, c0.c0.c1, c0.c1.c0, ..., c1.c2.c1 of Fp12 = Fp6[w]/(w^2 - v),
+ * Fp6 = Fp2[v]/(v^3 - (u + 1)). */
+int bb_diag_multi_pairing(bb_ctx* ctx, size_t n, const void* g1, const void* g2, void* gt_out);
+/* k of the G_T convention: bb_diag_multi_pairing returns e(P, Q)^k for the pairing e = f_{|x|,Q}(P)^((p^12 - 1) / r) */
+int bb_diag_gt_exponent(void);
+/* element-wise on n Fp12 values (12 Montgomery Fp each, tower order): op 0 a*b, 1 a^2, 2 1/a, 3 cyclotomic squaring of a,
+ * 4 a^p, 5 a^(p^2), 6 the final exponentiation a^(3 (p^12 - 1) / r), 7 a times the sparse line (b.c0.c0 + b.c0.c1 v) + (b.c1.c1 v) w */
+int bb_diag_fp12(bb_ctx* ctx, int op, const void* a, const void* b, void* out, size_t n);
+/* bb_groth16_verify_batch, also writing the G_T value its verdict was taken from (format of bb_diag_multi_pairing) */
+int bb_diag_verify_batch_gt(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* batch, const void* z, void* gt_out);
+/* a synthetic verifying key and n valid proofs from trapdoor scalars drawn from `seed`:
+ * alpha, beta, gamma, delta, ic_j = [t_j] G1 (j <= n_inputs); proof i: A = [a_i] G1, B = [b_i] G2,
+ * C = [(a_i b_i - alpha beta - gamma sum_j x_ij t_j) / delta] G1 (x_i0 = 1), all by fixed-base multiplication on the device.
+ * Key parts to host buffers (ic: n_inputs + 1 points); d_a, d_b, d_c, d_inputs (Montgomery Fr, n x n_inputs): device. */
+int bb_synth_proof_batch(bb_ctx* ctx, uint64_t seed, size_t n, size_t n_inputs, void* alpha_g1, void* beta_g2, void* gamma_g2,
+                         void* delta_g2, void* ic, void* d_a, void* d_b, void* d_c, void* d_inputs);
+
 #ifdef __cplusplus
 }
 #endif

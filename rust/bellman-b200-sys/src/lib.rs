@@ -10,6 +10,7 @@ use std::os::raw::{c_char, c_int, c_long, c_void};
 #[repr(C)] pub struct bb_msm_job { _private: [u8; 0] }
 #[repr(C)] pub struct bb_crs { _private: [u8; 0] }
 #[repr(C)] pub struct bb_prove { _private: [u8; 0] }
+#[repr(C)] pub struct bb_vk { _private: [u8; 0] }
 
 // bb_status
 pub const BB_OK: c_int = 0;
@@ -17,6 +18,8 @@ pub const BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE: c_int = 1;
 pub const BB_ERR_UNEXPECTED_IDENTITY: c_int = 2;
 pub const BB_ERR_IO_UNEXPECTED_EOF: c_int = 3;
 pub const BB_ERR_DENSITY_MISMATCH: c_int = 5;
+pub const BB_ERR_INVALID_VERIFYING_KEY: c_int = 6;
+pub const BB_ERR_INVALID_PROOF: c_int = 7;
 pub const BB_ERR_ARG: c_int = 16;
 pub const BB_ERR_CUDA: c_int = 17;
 pub const BB_ERR_NO_DEVICE: c_int = 18;
@@ -54,6 +57,20 @@ pub struct bb_witness {
     pub input_assignment: *const c_void, pub n_inputs: usize,
     pub aux_assignment: *const c_void, pub n_aux: usize,
     pub a_aux_density: *const u64, pub b_input_density: *const u64, pub b_aux_density: *const u64,
+    pub on_device: c_int,
+}
+
+#[repr(C)]
+pub struct bb_vk_desc {
+    pub alpha_g1: *const c_void,
+    pub beta_g2: *const c_void, pub gamma_g2: *const c_void, pub delta_g2: *const c_void,
+    pub ic: *const c_void, pub ic_len: usize,
+}
+
+#[repr(C)]
+pub struct bb_proof_batch {
+    pub a: *const c_void, pub b: *const c_void, pub c: *const c_void, pub n: usize,
+    pub inputs: *const c_void, pub n_inputs: usize,
     pub on_device: c_int,
 }
 
@@ -122,6 +139,12 @@ extern "C" {
                                     static_in: *const u8, proof: *mut u8) -> c_int;
     pub fn bb_groth16_prove(ctx: *mut bb_ctx, crs: *const bb_crs, w: *const bb_witness, r: *const u8, s: *const u8,
                             proof: *mut u8) -> c_int;
+
+    pub fn bb_vk_prepare(ctx: *mut bb_ctx, desc: *const bb_vk_desc, out: *mut *mut bb_vk) -> c_int;
+    pub fn bb_vk_destroy(vk: *mut bb_vk);
+    pub fn bb_groth16_verify(ctx: *mut bb_ctx, vk: *const bb_vk, a: *const c_void, b: *const c_void, c: *const c_void,
+                             inputs: *const c_void, n_inputs: usize) -> c_int;
+    pub fn bb_groth16_verify_batch(ctx: *mut bb_ctx, vk: *const bb_vk, batch: *const bb_proof_batch, z: *const c_void) -> c_int;
 
     pub fn bb_tuning_count() -> c_int;
     pub fn bb_tuning_name(index: c_int) -> *const c_char;

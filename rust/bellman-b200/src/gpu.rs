@@ -8,12 +8,13 @@ use std::os::raw::c_void;
 use std::ptr;
 use std::sync::Arc;
 
-use bellman::groth16::{Parameters, Proof};
-use bellman::SynthesisError;
+use bellman::groth16::{Parameters, Proof, VerifyingKey};
+use bellman::{SynthesisError, VerificationError};
 use bellman_b200_sys::*;
 use bls12_381::{Bls12, G1Affine, G1Projective, G2Affine, G2Projective, Scalar};
-use ff::PrimeField;
+use ff::{Field, PrimeField};
 use group::{prime::PrimeCurveAffine, Curve, UncompressedEncoding};
+use rand_core::{CryptoRng, RngCore};
 
 fn last_error() -> String {
     unsafe { CStr::from_ptr(bb_last_error()).to_string_lossy().into_owned() }
@@ -237,6 +238,79 @@ pub fn create_proof_b200(w: &WitnessView, crs: &GpuParameters, r: Scalar, s: Sca
     let mut bytes = [0u8; 192];
     status(unsafe { bb_groth16_prove(crs.ctx, crs.handle, &wit, r.to_repr().as_ptr(), s.to_repr().as_ptr(), bytes.as_mut_ptr()) })?;
     Proof::read(&bytes[..]).map_err(Into::into)               // the same 192 bytes Proof::write emits (lib.rs:39-45)
+}
+
+/// `PreparedVerifyingKey` (groth16/src/lib.rs:400-409, verifier.rs:11-21): the verifying key resident on the device.
+pub struct GpuVerifyingKey { pub(crate) ctx: *mut bb_ctx, pub(crate) handle: *mut bb_vk }
+unsafe impl Send for GpuVerifyingKey {}
+unsafe impl Sync for GpuVerifyingKey {}
+
+fn flat<A: B200Affine>(v: &[A]) -> Vec<u64> {
+    let mut f = vec![0u64; v.len() * A::WORDS];
+    for (p, out) in v.iter().zip(f.chunks_mut(A::WORDS)) { p.to_b200(out); }
+    f
+}
+
+/// bb_status of the verifier -> VerificationError (src/lib.rs:353-358); other statuses are back-end failures
+fn verification_status(rc: i32) -> Result<(), VerificationError> {
+    match rc {
+        BB_OK => Ok(()),
+        BB_ERR_INVALID_VERIFYING_KEY => Err(VerificationError::InvalidVerifyingKey),
+        BB_ERR_INVALID_PROOF => Err(VerificationError::InvalidProof),
+        _ => panic!("bellman_b200 verifier failed: {}", last_error()),
+    }
+}
+
+impl GpuVerifyingKey {
+    /// prepare_verifying_key (verifier.rs:11-21)
+    pub fn prepare(worker: &GpuWorker, vk: &VerifyingKey<Bls12>) -> Result<Self, SynthesisError> {
+        let (alpha, beta, gamma, delta) = (flat(&[vk.alpha_g1]), flat(&[vk.beta_g2]), flat(&[vk.gamma_g2]), flat(&[vk.delta_g2]));
+        let ic = flat(&vk.ic[..]);
+        let desc = bb_vk_desc {
+            alpha_g1: alpha.as_ptr() as _, beta_g2: beta.as_ptr() as _, gamma_g2: gamma.as_ptr() as _, delta_g2: delta.as_ptr() as _,
+            ic: ic.as_ptr() as _, ic_len: vk.ic.len(),
+        };
+        let mut handle = ptr::null_mut();
+        status(unsafe { bb_vk_prepare(worker.ctx, &desc, &mut handle) })?;
+        Ok(GpuVerifyingKey { ctx: worker.ctx, handle })
+    }
+}
+impl Drop for GpuVerifyingKey {
+    fn drop(&mut self) { unsafe { bb_vk_destroy(self.handle) } }
+}
+
+/// Drop-in for `groth16::verify_proof` (verifier.rs:23-58).
+pub fn verify_proof_b200(pvk: &GpuVerifyingKey, proof: &Proof<Bls12>, public_inputs: &[Scalar]) -> Result<(), VerificationError> {
+    let (a, b, c) = (flat(&[proof.a]), flat(&[proof.b]), flat(&[proof.c]));
+    verification_status(unsafe {
+        bb_groth16_verify(pvk.ctx, pvk.handle, a.as_ptr() as _, b.as_ptr() as _, c.as_ptr() as _, public_inputs.as_ptr() as _,
+                          public_inputs.len())
+    })
+}
+
+/// Drop-in for `batch::Verifier::verify` (verifier/batch.rs:100-173) over queued `(proof, inputs)` items: the random
+/// z_i come from `rng` (non-zero, batch.rs:124-129) and are passed canonical; all items must have as many inputs as the key
+/// expects, otherwise InvalidVerifyingKey, before any device work.
+pub fn batch_verify_b200<R: RngCore + CryptoRng>(worker: &GpuWorker, vk: &GpuVerifyingKey, items: &[(Proof<Bls12>, Vec<Scalar>)],
+                                                 mut rng: R) -> Result<(), VerificationError> {
+    let n_inputs = items.first().map_or(0, |(_, x)| x.len());
+    if items.iter().any(|(_, x)| x.len() != n_inputs) { return Err(VerificationError::InvalidVerifyingKey); }
+    let (mut a, mut b, mut c) = (Vec::with_capacity(items.len() * 12), Vec::with_capacity(items.len() * 24), Vec::with_capacity(items.len() * 12));
+    let mut inputs: Vec<Scalar> = Vec::with_capacity(items.len() * n_inputs);
+    let mut z: Vec<u8> = Vec::with_capacity(items.len() * 32);
+    for (proof, x) in items {
+        a.extend(flat(&[proof.a]));
+        b.extend(flat(&[proof.b]));
+        c.extend(flat(&[proof.c]));
+        inputs.extend_from_slice(x);
+        let zi = loop { let v = Scalar::random(&mut rng); if !bool::from(v.is_zero()) { break v; } };
+        z.extend_from_slice(zi.to_repr().as_ref());
+    }
+    let batch = bb_proof_batch {
+        a: a.as_ptr() as _, b: b.as_ptr() as _, c: c.as_ptr() as _, n: items.len(),
+        inputs: inputs.as_ptr() as _, n_inputs, on_device: 0,
+    };
+    verification_status(unsafe { bb_groth16_verify_batch(worker.ctx, vk.handle, &batch, z.as_ptr() as _) })
 }
 
 #[allow(dead_code)]
