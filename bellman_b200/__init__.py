@@ -678,3 +678,5 @@ def fr_dot_device(worker, d_a, d_b, n):
 # groth16 verification (groth16/src/verifier.rs, verifier/batch.rs)
 from .verifier import (BatchVerifier, InvalidProof, InvalidVerifyingKey, PreparedVerifyingKey,  # noqa: E402
                        VerificationError, prepare_verifying_key, verify_proof)
+# Proof::read / Proof::write over a batch (groth16/src/lib.rs:39-99)
+from .verifier import InvalidProofEncoding, read_proof, read_proofs, write_proofs  # noqa: E402

@@ -8,12 +8,18 @@ bb_groth16_verify_batch.
 
 Proofs are ABI-format affine point arrays (A, C: 12 u64, B: 24 u64); public inputs are Fr, either
 Python integers or an (L, 4) uint64 array in Montgomery form.
+
+Proofs as bytes (Proof::read / Proof::write, groth16/src/lib.rs:39-99, over bb_proofs_read / bb_proofs_write):
+
+    a, b, c, status = read_proofs(worker, data, stride=384)     # status: one byte per proof, 0 = valid
+    proof = read_proof(worker, b192)                           # raises InvalidProofEncoding like Proof::read
+    bv.queue_bytes((b192, inputs)); bv.verify(rng, pvk)        # decoded on the device at verify() time
 """
 import ctypes as C
 
 import numpy as np
 
-from . import EvaluationDomain, _c64, _check, _ERRORS, _ptr, load_library
+from . import EvaluationDomain, _addr, _c64, _check, _ERRORS, _ptr, load_library
 
 
 class VerificationError(Exception):
@@ -135,6 +141,103 @@ def verify_batch_arrays(pvk, a, b, c, inputs, z=None, on_device=False, n=None, n
     return True, out
 
 
+class InvalidProofEncoding(ValueError):
+    """Proof::read failed (groth16/src/lib.rs:47-99): bellman's io::Error of kind InvalidData.  The message starts with
+    bellman's text ("invalid G1", "invalid G2" or "point at infinity"); `status` is the byte of bb_proofs_read and
+    `index` the proof's position (in the queue, for BatchVerifier.queue_bytes)."""
+
+    def __init__(self, message, status=None, index=None):
+        super().__init__(message)
+        self.status, self.index = status, index
+
+
+# the status byte of bb_proofs_read: (which << 4) | why
+READ_OK, READ_BAD_FLAGS, READ_NON_CANONICAL, READ_NOT_ON_CURVE, READ_NOT_IN_SUBGROUP, READ_IDENTITY = range(6)
+PROOF_BYTES = 192
+
+
+def read_error_message(status):
+    """bellman's io::Error text for a non-zero status byte"""
+    if status & 15 == READ_IDENTITY:
+        return "point at infinity"
+    return "invalid G2" if status >> 4 == 2 else "invalid G1"
+
+
+class _ProofBytes(C.Structure):
+    _fields_ = [("bytes", C.c_void_p), ("n", C.c_size_t), ("stride", C.c_size_t), ("on_device", C.c_int)]
+
+
+def read_proofs(worker, data, n=None, stride=PROOF_BYTES, on_device=False, out_device=None):
+    """Proof::read over a batch on the device (bb_proofs_read).  Proof i is the 192 bytes at data[i * stride:].
+    data: bytes-like or a uint8 array (host), or with on_device=True a device address (then n is required).
+    n: number of proofs (default: every whole record of data).  out_device: None, or three device addresses (n x 96 B,
+    n x 192 B, n x 96 B) that receive A, B, C.  Returns (a, b, c, status): the points as (n, 12) / (n, 24) / (n, 12)
+    uint64 arrays (ABI format) or the three device addresses, and the (n,) uint8 status bytes."""
+    lib = load_library()
+    pb = _ProofBytes()
+    keep = None
+    if on_device:
+        if n is None:
+            raise ValueError("read_proofs: n is required for bytes in device memory")
+        pb.bytes = _addr(data)
+    else:
+        keep = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, np.uint8).reshape(-1)
+        whole = 0 if keep.size < PROOF_BYTES or stride < PROOF_BYTES else 1 + (keep.size - PROOF_BYTES) // stride
+        n = whole if n is None else n
+        if n > whole:
+            raise ValueError(f"read_proofs: {keep.size} bytes hold {whole} proofs at stride {stride}, not {n}")
+        pb.bytes = keep.ctypes.data if keep.size else None
+    pb.n, pb.stride, pb.on_device = n, stride, 1 if on_device else 0
+    status = np.zeros(max(n, 1), np.uint8)
+    n_invalid = C.c_size_t()
+    if out_device is not None:
+        da, db, dc = (C.c_void_p(_addr(p)) for p in out_device)
+        _check(lib.bb_proofs_read(worker._h, C.byref(pb), da, db, dc, C.c_int(1), _ptr(status), C.byref(n_invalid)))
+        return out_device[0], out_device[1], out_device[2], status[:n]
+    a, b, c = np.zeros((n, 12), np.uint64), np.zeros((n, 24), np.uint64), np.zeros((n, 12), np.uint64)
+    _check(lib.bb_proofs_read(worker._h, C.byref(pb), _ptr(a), _ptr(b), _ptr(c), C.c_int(0), _ptr(status), C.byref(n_invalid)))
+    return a, b, c, status[:n]
+
+
+def read_proof(worker, b192):
+    """Proof::read of one proof: the ABI triple (a, b, c), or InvalidProofEncoding with bellman's message"""
+    if len(b192) != PROOF_BYTES:
+        raise ValueError("a proof is 192 bytes")
+    a, b, c, status = read_proofs(worker, bytes(b192), n=1)
+    if status[0]:
+        raise InvalidProofEncoding(read_error_message(int(status[0])), status=int(status[0]), index=0)
+    return a[0], b[0], c[0]
+
+
+def write_proofs(worker, a, b, c):
+    """Proof::write over a batch on the device (bb_proofs_write): ABI point arrays -> n x 192 bytes"""
+    a, b, c = _c64(a, 12), _c64(b, 24), _c64(c, 12)
+    n = a.shape[0]
+    assert b.shape[0] == n and c.shape[0] == n
+    out = np.zeros(max(n, 1) * PROOF_BYTES, np.uint8)
+    _check(load_library().bb_proofs_write(worker._h, _ptr(a), _ptr(b), _ptr(c), C.c_size_t(n), C.c_int(0), _ptr(out)))
+    return bytes(out[:n * PROOF_BYTES])
+
+
+def write_proofs_device(worker, d_a, d_b, d_c, n, d_out):
+    """bb_proofs_write with everything in HBM: n proofs of the device arrays d_a, d_b, d_c -> d_out (n x 192 B)"""
+    ptrs = (C.c_void_p(_addr(p)) for p in (d_a, d_b, d_c))
+    _check(load_library().bb_proofs_write(worker._h, *ptrs, C.c_size_t(n), C.c_int(1), C.c_void_p(_addr(d_out))))
+
+
+def points_decompress(worker, group, data, check_subgroup=True):
+    """diagnostic (bb_diag_points_decompress): from_compressed, or from_compressed_unchecked with check_subgroup=False,
+    of packed 48-byte (G1) or 96-byte (G2) encodings -> ((n, 12 | 24) uint64 points, (n,) uint8 codes)"""
+    enc, width = (48, 12) if group == 1 else (96, 24)
+    buf = np.frombuffer(bytes(data), np.uint8)
+    n = buf.size // enc
+    out = np.zeros((n, width), np.uint64)
+    why = np.zeros(max(n, 1), np.uint8)
+    _check(load_library().bb_diag_points_decompress(worker._h, C.c_int(group), _ptr(buf) if n else None, C.c_size_t(n),
+                                                    C.c_int(1 if check_subgroup else 0), _ptr(out), _ptr(why)))
+    return out, why[:n]
+
+
 class BatchVerifier:
     """groth16::batch::Verifier (batch.rs:72-173)."""
 
@@ -146,10 +249,21 @@ class BatchVerifier:
         proof, inputs = item
         self.items.append(((_c64(proof[0], 12), _c64(proof[1], 24), _c64(proof[2], 12)), fr_inputs(inputs)))
 
+    def queue_bytes(self, proof_bytes, inputs):
+        """queue a proof in its 192-byte Proof::write encoding.  It is read on the device at verify() time, together with
+        every other proof queued this way (one bb_proofs_read), and its points stay there for the verification."""
+        if len(proof_bytes) != PROOF_BYTES:
+            raise ValueError("a proof is 192 bytes")
+        self.items.append((bytes(proof_bytes), fr_inputs(inputs)))
+
     def verify(self, rng, pvk):
         """batch.rs:100-173 against a PreparedVerifyingKey.  rng: None = z from the operating system (getrandom); any
-        object with randrange gives reproducible z.  Returns None; raises InvalidProof or InvalidVerifyingKey."""
+        object with randrange gives reproducible z.  Returns None; raises InvalidProof or InvalidVerifyingKey, and
+        InvalidProofEncoding (naming the queue index) for a proof of queue_bytes that does not read -- before any pairing
+        work, as bellman's Proof::read fails before its proof could be queued."""
         n = len(self.items)
+        if any(isinstance(p, bytes) for p, _ in self.items):
+            return self._verify_from_bytes(rng, pvk)
         if n and any(x.shape[0] + 1 != pvk.ic_len for _, x in self.items):
             raise InvalidVerifyingKey(f"[bb_status 6] InvalidVerifyingKey: a key with {pvk.ic_len} ic entries")
         L = pvk.ic_len - 1
@@ -159,6 +273,35 @@ class BatchVerifier:
         x = np.stack([xi.reshape(L, 4) for _, xi in self.items]) if n and L else np.zeros((n, max(L, 0), 4), np.uint64)
         z = None if rng is None else [rng.randrange(1, R_MODULUS) for _ in range(n)]
         verify_batch_arrays(pvk, a, b, c, x, z, n_inputs=max(L, 0))
+
+    def _verify_from_bytes(self, rng, pvk):
+        """the batch in device buffers: the queue_bytes proofs first (decoded in place), then the queue() ones (uploaded);
+        the verdict of a batch does not depend on the order of its items"""
+        worker, n, L = pvk.worker, len(self.items), pvk.ic_len - 1
+        enc = [i for i, (p, _) in enumerate(self.items) if isinstance(p, bytes)]
+        dec = [i for i, (p, _) in enumerate(self.items) if not isinstance(p, bytes)]
+        nb = len(enc)
+        d = {"a": worker.device_alloc(n * 96), "b": worker.device_alloc(n * 192), "c": worker.device_alloc(n * 96),
+             "x": worker.device_alloc(max(1, n * max(L, 0)) * 32)}
+        try:
+            _, _, _, status = read_proofs(worker, b"".join(self.items[i][0] for i in enc), n=nb, out_device=(d["a"], d["b"], d["c"]))
+            bad = np.flatnonzero(status)
+            if bad.size:
+                k = int(bad[0])
+                raise InvalidProofEncoding(f"{read_error_message(int(status[k]))} (queued proof {enc[k]})", status=int(status[k]), index=enc[k])
+            if any(x.shape[0] + 1 != pvk.ic_len for _, x in self.items):
+                raise InvalidVerifyingKey(f"[bb_status 6] InvalidVerifyingKey: a key with {pvk.ic_len} ic entries")
+            if dec:
+                for key, k, width in (("a", 0, 12), ("b", 1, 24), ("c", 2, 12)):
+                    rows = np.stack([self.items[i][0][k].reshape(width) for i in dec])
+                    worker.upload(C.c_void_p(_addr(d[key]) + nb * width * 8), rows)
+            if L:
+                worker.upload(d["x"], np.stack([self.items[i][1].reshape(L, 4) for i in enc + dec]))
+            z = None if rng is None else [rng.randrange(1, R_MODULUS) for _ in range(n)]
+            verify_batch_arrays(pvk, d["a"], d["b"], d["c"], d["x"], z, on_device=True, n=n, n_inputs=L)
+        finally:
+            for p in d.values():
+                worker.device_free(p)
 
 
 def multi_pairing(worker, g1, g2):

@@ -11,6 +11,10 @@ HBM, `e2e` the same batch from pinned host buffers.  Outside the timed regions t
 accepted and that the same batch with C_0 replaced by C_1 is rejected.  The line carries the per-stage device
 milliseconds (CUDA events of the library's profile mode) and the Fp-multiplication rate of the Miller loops.
 
+--from-bytes adds a `from_bytes` object: proofs/s of decode + verify with the batch as 192-byte Proof::write encodings
+in pinned host memory (bb_proofs_read into HBM, then the batch verifier), the decode.* stage milliseconds and the bytes
+copied to the device per step.  Without it the line is exactly the one above.
+
 --dump-outputs DIR writes the two verdicts and the G_T value of the rejected batch (deterministic under the seeded z)
 as float64 .npy files, the format of bench.py --dump-outputs.  Prints one JSON line on stdout; writes nothing else.
 """
@@ -44,6 +48,8 @@ def parse():
     ap.add_argument("--log-size", type=int, default=DEFAULT_LOG, help="log2 of the proofs per batch")
     ap.add_argument("--inputs", type=int, default=DEFAULT_INPUTS, help="public inputs per proof")
     ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the verdicts and the rejected batch's G_T value as DIR/<name>.npy")
+    ap.add_argument("--from-bytes", action="store_true",
+                    help="also time decode + verify of the batch as 192-byte Proof::write encodings in pinned host memory (adds `from_bytes`)")
     return ap.parse_args()
 
 
@@ -55,6 +61,58 @@ def miller_fp_muls_per_pair():
     dbl = 5 * 2 + 3 * 2 + 4 * 3                             # miller_dbl_step: 5 Fp2 squarings, 3 Fp2 x Fp, 4 Fp2 products
     add = 11 * 3 + 3 * 2 + 2 * 2                            # miller_add_step: 11 Fp2 products, 3 Fp2 x Fp, 2 Fp2 squarings
     return 63 * (fp12_sqr + dbl + mul_line) + 5 * (add + mul_line)
+
+
+DECODE_STAGES = ("decode.upload", "decode.g1", "decode.g2", "decode.status", "decode.download")
+
+
+def from_bytes_leg(args, worker, pvk, d, host, z, timed):
+    """--from-bytes: the batch as n x 192 bytes (bb_proofs_write on the device) in pinned host memory; a step is one
+    bb_proofs_read into device buffers plus the batch verification of the decoded points.  Outside the timed region: the
+    decoded points equal the synthetic batch, and one flipped x byte of B at the middle proof is reported there."""
+    import torch
+
+    from bellman_b200 import verifier as V
+    n, L = host["a"].shape[0], args.inputs
+    d_bytes = worker.device_alloc(n * 192)
+    V.write_proofs_device(worker, d["a"], d["b"], d["c"], n, d_bytes)
+    keep = torch.zeros(n * 192, dtype=torch.uint8).pin_memory()
+    data = keep.numpy()
+    worker.download(d_bytes, data)
+    worker.device_free(d_bytes)
+    out = {k: worker.device_alloc(n * w * 8) for k, w in (("a", 12), ("b", 24), ("c", 12))}
+    dev = (out["a"], out["b"], out["c"])
+
+    def step_bytes():
+        _, _, _, status = V.read_proofs(worker, data, n=n, out_device=dev)
+        if status.any():
+            raise AssertionError(f"{int((status != 0).sum())} proofs of the timed batch do not read")
+        V.verify_batch_arrays(pvk, *dev, d["x"], z=z, on_device=True, n=n, n_inputs=L)
+
+    worker.set_option("profile", 1)
+    dt, _, h2d = timed(step_bytes)
+    decode = {s.split(".")[1]: worker.profile_read(s)[0] / args.steps for s in DECODE_STAGES}
+    worker.set_option("profile", 0)
+    same = True
+    for key, w in (("a", 12), ("b", 24), ("c", 12)):
+        got = np.zeros((n, w), np.uint64)
+        worker.download(out[key], got)
+        same = same and np.array_equal(got, host[key])
+    mid = n // 2
+    bad = data.copy()
+    bad[192 * mid + 48 + 95] ^= 1                               # the last byte of x.c0 of B
+    _, _, _, status = V.read_proofs(worker, bad, n=n)
+    flagged = np.flatnonzero(status)
+    reported = flagged.tolist() == [mid] and int(status[mid]) >> 4 == 2
+    for p in out.values():
+        worker.device_free(p)
+    return {"value": n * args.steps / dt, "unit": "proofs/s", "ms_per_step": 1e3 * dt / args.steps,
+            "decode_ms": round(sum(decode.values()), 3), "decode_stages_ms": {k: round(v, 3) for k, v in decode.items()},
+            "h2d_bytes_per_step": int(h2d),
+            "source": "the timed batch as Proof::write bytes (bb_proofs_write on the device) in pinned host memory; "
+                      "step = bb_proofs_read into HBM + bb_groth16_verify_batch on the decoded points",
+            "checks": {"decoded_points": "equal" if same else "DIFFERENT", "corrupted_b_at_middle": "reported" if reported else "MISSED"},
+            "corrupted": {"index": mid, "status": int(status[mid])}}
 
 
 def run(args):
@@ -125,6 +183,7 @@ def run(args):
     c_bad[0] = host["c"][1 % n]
     ok_bad, gt_bad = V.verify_batch_arrays(pvk, host["a"], host["b"], c_bad, host["x"], z=z, n_inputs=L, gt=True)
     checks = {"timed_batch": "accepted" if ok else "REJECTED", "one_c_replaced": "rejected" if not ok_bad else "ACCEPTED"}
+    from_bytes = from_bytes_leg(args, worker, pvk, d, host, z, timed) if args.from_bytes else None
     per_pair = miller_fp_muls_per_pair()
     miller_ms = stages["miller"]
     line = {"metric": "groth16_batch_verify_proofs_per_sec", "value": n * args.steps / dt_val, "unit": "proofs/s", "n_gpus": 1,
@@ -145,9 +204,13 @@ def run(args):
                        "model": "miller_fp_muls_per_pair(): 63 doubling and 5 addition steps of csrc/tower.cuh counted in Fp products"},
             "cpu_baseline": None,
             "cpu_baseline_reason": "oracle-1 has no CPU pairing; the Python pairing of oracle-0 is a correctness reference, not a timed baseline"}
+    if from_bytes is not None:
+        line["from_bytes"] = from_bytes
     bench.dump_outputs(args.dump_outputs, {"verdicts": np.array([int(ok), int(ok_bad)], np.uint32), "gt_tampered": gt_bad})
     bench.emit(line)
     assert ok and not ok_bad, checks
+    if from_bytes is not None:
+        assert from_bytes["checks"] == {"decoded_points": "equal", "corrupted_b_at_middle": "reported"}, from_bytes["checks"]
     pvk.free()
     for p in d.values():
         worker.device_free(p)

@@ -85,7 +85,7 @@ void bb_ctx_destroy(bb_ctx* ctx);
  *   msm_precompute_groups  which vectors use the tables: mask of 1 (G1) and 2 (G2), default 3
  *   shard_windows      multi-GPU: window groups per base range (default 4; 1 = base ranges only)
  *   ntt_radix8         1 = register radix-8 NTT windows (default 0: measured slower), ntt_tile_log, ntt_col_bits
- *   profile            1 = CUDA-event timing of the MSM stages (bb_profile_read) */
+ *   profile            1 = CUDA-event timing of the MSM stages, and of the verify.* and decode.* stages (bb_profile_read) */
 int bb_ctx_set_option(bb_ctx* ctx, const char* key, long value);
 int bb_ctx_synchronize(bb_ctx* ctx);
 /* counters for the harness: number of kernels this context has launched */
@@ -298,6 +298,37 @@ int bb_groth16_verify(bb_ctx* ctx, const bb_vk* vk, const void* a, const void* b
  * z: n canonical 32-byte scalars in [1, r) (zero or >= r: BB_ERR_ARG), or NULL = drawn from the operating system
  * (getrandom, zeros redrawn).  The key check comes first, before any device work.  An empty batch is accepted. */
 int bb_groth16_verify_batch(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* batch, const void* z);
+
+/* ---- reading and writing proofs: Proof::read / Proof::write (groth16/src/lib.rs:39-99) -------------------------
+ * A proof is 192 bytes: compressed A (48 B), B (96 B), C (48 B), the ZCash encoding of bls12_381 0.8.  Decoding runs
+ * on the device, one thread per point, in variable time (proof bytes are public).  For each proof A, then B, then C
+ * is read; the first element that fails decides the status byte:
+ *     status = 0 (valid) or (which << 4) | why,   which: 1 = A, 2 = B, 3 = C
+ *     why  check, in this priority                                                 bellman's io::Error (InvalidData)
+ *      1   compression bit (0x80 of byte 0) clear; or infinity bit (0x40) set       "invalid G1" / "invalid G2"
+ *          with the sort bit (0x20) or any bit of x set
+ *      2   x >= p (G2: x.c1 in bytes 0-47 below the flags, or x.c0 in bytes 48-95)  "invalid G1" / "invalid G2"
+ *      3   x^3 + b has no square root (not on the curve)                            "invalid G1" / "invalid G2"
+ *      4   the point is not in the order-r subgroup                                 "invalid G1" / "invalid G2"
+ *      5   a valid encoding of the identity (0xC0, then zeros)                      "point at infinity"
+ * y is the square root whose "lexicographically largest" flag (G1: y > (p-1)/2; G2: y.c1 decides, y.c0 if y.c1 = 0)
+ * equals the sort bit.  All three points of an invalid proof are written as the identity (zeros). */
+#define BB_PROOF_BYTES 192
+#define BB_PROOF_WHICH(status) ((status) >> 4)
+#define BB_PROOF_WHY(status) ((status) & 15)
+enum { BB_READ_OK = 0, BB_READ_BAD_FLAGS = 1, BB_READ_NON_CANONICAL = 2, BB_READ_NOT_ON_CURVE = 3, BB_READ_NOT_IN_SUBGROUP = 4,
+       BB_READ_IDENTITY = 5 };
+/* Proof::read (groth16/src/lib.rs:47-99) over n proofs; proof i at bytes + i*stride (stride 0 = 192); no alignment is
+ * assumed.  on_device != 0: bytes is a device pointer; otherwise only the 192 proof bytes of each record are copied. */
+typedef struct bb_proof_bytes { const void* bytes; size_t n; size_t stride; int on_device; } bb_proof_bytes;
+/* a, c: n x 96 B, b: n x 192 B, device pointers if out_on_device else host; status: n bytes, host, always written;
+ * *n_invalid = number of non-zero statuses.  BB_OK whenever the call ran, even if some proofs are invalid.
+ * BB_ERR_ARG: a NULL pointer with n > 0, or 0 < stride < 192. */
+int bb_proofs_read(bb_ctx* ctx, const bb_proof_bytes* in, void* a, void* b, void* c, int out_on_device,
+                   uint8_t* status, size_t* n_invalid);
+/* Proof::write (lib.rs:39-45) over n proofs: out = n x 192 B (a, b, c and out are device pointers if on_device).
+ * Byte for byte what bb_point_compress gives for each point. */
+int bb_proofs_write(bb_ctx* ctx, const void* a, const void* b, const void* c, size_t n, int on_device, void* out);
 
 /* ---- tuning per key ------------------------------------------------------------------------
  * The MSM has several forms with identical results (per-window bucket sets; one bucket set over resident window

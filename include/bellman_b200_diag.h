@@ -61,6 +61,12 @@ int bb_diag_verify_batch_gt(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* 
 int bb_synth_proof_batch(bb_ctx* ctx, uint64_t seed, size_t n, size_t n_inputs, void* alpha_g1, void* beta_g2, void* gamma_g2,
                          void* delta_g2, void* ic, void* d_a, void* d_b, void* d_c, void* d_inputs);
 
+/* ---- decoding (decode.cu) ------------------------------------------------------------------------------------- */
+/* from_compressed (check_subgroup != 0) or from_compressed_unchecked (check_subgroup = 0) of n packed points of `group`
+ * (48 or 96 B each, host memory) on the device.  out: n affine points in the ABI format (zeros unless why = 0); why: n
+ * bytes, the codes of bb_proofs_read (5 = the identity, a valid encoding that Proof::read rejects). */
+int bb_diag_points_decompress(bb_ctx* ctx, int group, const void* bytes, size_t n, int check_subgroup, void* out, uint8_t* why);
+
 #ifdef __cplusplus
 }
 #endif

@@ -74,6 +74,20 @@ pub struct bb_proof_batch {
     pub on_device: c_int,
 }
 
+// Proof::read status byte: (which << 4) | why, which 1 = A, 2 = B, 3 = C
+pub const BB_PROOF_BYTES: usize = 192;
+pub const BB_READ_OK: u8 = 0;
+pub const BB_READ_BAD_FLAGS: u8 = 1;
+pub const BB_READ_NON_CANONICAL: u8 = 2;
+pub const BB_READ_NOT_ON_CURVE: u8 = 3;
+pub const BB_READ_NOT_IN_SUBGROUP: u8 = 4;
+pub const BB_READ_IDENTITY: u8 = 5;
+
+#[repr(C)]
+pub struct bb_proof_bytes {
+    pub bytes: *const c_void, pub n: usize, pub stride: usize, pub on_device: c_int,
+}
+
 extern "C" {
     pub fn bb_last_error() -> *const c_char;
     pub fn bb_version() -> c_int;
@@ -145,6 +159,10 @@ extern "C" {
     pub fn bb_groth16_verify(ctx: *mut bb_ctx, vk: *const bb_vk, a: *const c_void, b: *const c_void, c: *const c_void,
                              inputs: *const c_void, n_inputs: usize) -> c_int;
     pub fn bb_groth16_verify_batch(ctx: *mut bb_ctx, vk: *const bb_vk, batch: *const bb_proof_batch, z: *const c_void) -> c_int;
+    pub fn bb_proofs_read(ctx: *mut bb_ctx, input: *const bb_proof_bytes, a: *mut c_void, b: *mut c_void, c: *mut c_void,
+                          out_on_device: c_int, status: *mut u8, n_invalid: *mut usize) -> c_int;
+    pub fn bb_proofs_write(ctx: *mut bb_ctx, a: *const c_void, b: *const c_void, c: *const c_void, n: usize, on_device: c_int,
+                           out: *mut c_void) -> c_int;
 
     pub fn bb_tuning_count() -> c_int;
     pub fn bb_tuning_name(index: c_int) -> *const c_char;

@@ -313,5 +313,98 @@ pub fn batch_verify_b200<R: RngCore + CryptoRng>(worker: &GpuWorker, vk: &GpuVer
     verification_status(unsafe { bb_groth16_verify_batch(worker.ctx, vk.handle, &batch, z.as_ptr() as _) })
 }
 
+/// bellman's io::Error of `Proof::read` (groth16/src/lib.rs:47-99) for a non-zero bb_proofs_read status byte
+fn read_error(st: u8) -> io::Error {
+    let msg = if st & 15 == BB_READ_IDENTITY { "point at infinity" } else if st >> 4 == 2 { "invalid G2" } else { "invalid G1" };
+    io::Error::new(io::ErrorKind::InvalidData, msg)
+}
+
+fn whole_proofs(len: usize, stride: usize) -> usize {
+    if len < BB_PROOF_BYTES { 0 } else { 1 + (len - BB_PROOF_BYTES) / stride }
+}
+
+/// Drop-in for `Proof::read` (groth16/src/lib.rs:47-99) over a batch, decoded on the device: proof i is the 192 bytes at
+/// `bytes[i * stride..]` (stride 0 = 192; e.g. 384 for Sapling spend descriptions sliced at the proof's offset 128), for
+/// every whole record.  Errors are the `InvalidData` io::Errors Proof::read returns ("invalid G1", "invalid G2",
+/// "point at infinity").
+pub fn read_proofs_b200(worker: &GpuWorker, bytes: &[u8], stride: usize) -> Vec<io::Result<Proof<Bls12>>> {
+    let stride = if stride == 0 { BB_PROOF_BYTES } else { stride };
+    assert!(stride >= BB_PROOF_BYTES, "a proof record is at least {} bytes", BB_PROOF_BYTES);
+    let n = whole_proofs(bytes.len(), stride);
+    let (mut a, mut b, mut c) = (vec![0u64; n * 12], vec![0u64; n * 24], vec![0u64; n * 12]);
+    let mut st = vec![0u8; n];
+    let mut n_invalid = 0usize;
+    let input = bb_proof_bytes { bytes: bytes.as_ptr() as _, n, stride, on_device: 0 };
+    let rc = unsafe {
+        bb_proofs_read(worker.ctx, &input, a.as_mut_ptr() as _, b.as_mut_ptr() as _, c.as_mut_ptr() as _, 0, st.as_mut_ptr(), &mut n_invalid)
+    };
+    if rc != BB_OK { panic!("bellman_b200 bb_proofs_read failed: {}", last_error()); }
+    (0..n).map(|i| {
+        if st[i] != 0 { return Err(read_error(st[i])); }
+        Ok(Proof { a: G1Affine::from_b200(&a[12 * i..12 * (i + 1)]), b: G2Affine::from_b200(&b[24 * i..24 * (i + 1)]),
+                   c: G1Affine::from_b200(&c[12 * i..12 * (i + 1)]) })
+    }).collect()
+}
+
+/// What `batch_verify_bytes_b200` fails with: a proof that does not read (its index and the io::Error of `Proof::read`),
+/// or the `VerificationError` of the batch.
+#[derive(Debug)]
+pub enum BytesBatchError { Read { index: usize, error: io::Error }, Verification(VerificationError) }
+
+/// A device buffer of the context's allocator, freed on drop.
+struct DeviceBuf { ctx: *mut bb_ctx, p: *mut c_void }
+impl DeviceBuf {
+    fn new(ctx: *mut bb_ctx, bytes: usize) -> Self {
+        let mut p = ptr::null_mut();
+        if unsafe { bb_device_alloc(ctx, bytes.max(16), &mut p) } != BB_OK { panic!("bellman_b200 device allocation failed: {}", last_error()); }
+        DeviceBuf { ctx, p }
+    }
+}
+impl Drop for DeviceBuf {
+    fn drop(&mut self) { unsafe { bb_device_free(self.ctx, self.p); } }
+}
+
+/// `batch::Verifier::verify` over items queued as `Proof::write` bytes: one bb_proofs_read decodes every proof into device
+/// buffers and the batch verifier runs on them there, so the points never return to the host.  A proof that does not read
+/// is reported before any pairing work -- a bellman caller's `Proof::read` fails before the proof could be queued; only
+/// the first 192 bytes of each item are read, and a shorter item fails as `read_exact` does.  Otherwise the result is that
+/// of `batch_verify_b200`.
+pub fn batch_verify_bytes_b200<R: RngCore + CryptoRng>(worker: &GpuWorker, vk: &GpuVerifyingKey, items: &[(&[u8], Vec<Scalar>)],
+                                                       mut rng: R) -> Result<(), BytesBatchError> {
+    let n = items.len();
+    let mut bytes = Vec::with_capacity(n * BB_PROOF_BYTES);
+    for (index, (b, _)) in items.iter().enumerate() {
+        if b.len() < BB_PROOF_BYTES {
+            return Err(BytesBatchError::Read { index, error: io::Error::new(io::ErrorKind::UnexpectedEof, "failed to fill whole buffer") });
+        }
+        bytes.extend_from_slice(&b[..BB_PROOF_BYTES]);
+    }
+    let (d_a, d_b, d_c) = (DeviceBuf::new(worker.ctx, n * 96), DeviceBuf::new(worker.ctx, n * 192), DeviceBuf::new(worker.ctx, n * 96));
+    let mut st = vec![0u8; n];
+    let mut n_invalid = 0usize;
+    let input = bb_proof_bytes { bytes: bytes.as_ptr() as _, n, stride: BB_PROOF_BYTES, on_device: 0 };
+    let rc = unsafe { bb_proofs_read(worker.ctx, &input, d_a.p, d_b.p, d_c.p, 1, st.as_mut_ptr(), &mut n_invalid) };
+    if rc != BB_OK { panic!("bellman_b200 bb_proofs_read failed: {}", last_error()); }
+    if let Some(index) = st.iter().position(|&s| s != 0) {
+        return Err(BytesBatchError::Read { index, error: read_error(st[index]) });
+    }
+    let n_inputs = items.first().map_or(0, |(_, x)| x.len());
+    if items.iter().any(|(_, x)| x.len() != n_inputs) { return Err(BytesBatchError::Verification(VerificationError::InvalidVerifyingKey)); }
+    let mut inputs: Vec<Scalar> = Vec::with_capacity(n * n_inputs);
+    let mut z: Vec<u8> = Vec::with_capacity(n * 32);
+    for (_, x) in items {
+        inputs.extend_from_slice(x);
+        let zi = loop { let v = Scalar::random(&mut rng); if !bool::from(v.is_zero()) { break v; } };
+        z.extend_from_slice(zi.to_repr().as_ref());
+    }
+    let d_x = DeviceBuf::new(worker.ctx, inputs.len() * 32);
+    if !inputs.is_empty() && unsafe { bb_device_upload(worker.ctx, d_x.p, inputs.as_ptr() as _, inputs.len() * 32) } != BB_OK {
+        panic!("bellman_b200 upload failed: {}", last_error());
+    }
+    let batch = bb_proof_batch { a: d_a.p, b: d_b.p, c: d_c.p, n, inputs: d_x.p, n_inputs, on_device: 1 };
+    verification_status(unsafe { bb_groth16_verify_batch(worker.ctx, vk.handle, &batch, z.as_ptr() as _) })
+        .map_err(BytesBatchError::Verification)
+}
+
 #[allow(dead_code)]
 fn _projective_types_are_what_wait_returns(_: G1Projective, _: G2Projective) {}

@@ -78,6 +78,77 @@ _x = F.BLS_X
 assert (_x - 1) ** 2 * (_x + P_MOD) * (_x ** 2 + P_MOD ** 2 - 1) + 3 == 3 * (P_MOD ** 4 - P_MOD ** 2 + 1) // R_MOD
 assert (P_MOD ** 4 - P_MOD ** 2 + 1) % R_MOD == 0 and -_x == 0xD201000000010000
 
+# ---- decoding compressed points (decode.cu) ----
+# square roots: p = 3 mod 4, so sqrt(a) = a^((p+1)/4) in Fp; in Fp2 Algorithm 9 of eprint 2012/685 runs a^((p-3)/4) and
+# (1 + alpha)^((p-1)/2) -- the latter exponent is FP_HALF
+assert P_MOD % 4 == 3
+EXP_SQRT, EXP_SQRT2 = (P_MOD + 1) // 4, (P_MOD - 3) // 4
+# subgroup checks of eprint 2021/1130 (proofs for BLS12-381: eprint 2022/352):
+#   G1: phi(P) = -[x^2] P  with phi(x, y) = (beta x, y), beta the cube root of unity whose eigenvalue is -x^2
+#   G2: psi(P) = [x] P     with psi(x, y) = (conj(x) / xi^((p-1)/3), conj(y) / xi^((p-1)/2))
+_w = next(w for w in (pow(g, (P_MOD - 1) // 3, P_MOD) for g in range(2, 100)) if w != 1)
+
+
+def _mul_int(G, pt, k):                 # [k] pt for an integer k >= 0 WITHOUT reducing k mod r (pt may lie outside G1 / G2)
+    acc = None
+    while k:
+        if k & 1:
+            acc = G.add(acc, pt)
+        pt = G.add(pt, pt)
+        k >>= 1
+    return acc
+
+
+def _phi(pt):
+    return (BETA * pt[0] % P_MOD, pt[1])
+
+
+def _psi(pt):
+    (x0, x1), (y0, y1) = pt
+    return F.Fp2Ops.mul((x0, -x1 % P_MOD), PSI_X), F.Fp2Ops.mul((y0, -y1 % P_MOD), PSI_Y)
+
+
+def _g1_fast_check(pt):
+    return _phi(pt) == F.G1.neg(_mul_int(F.G1, pt, _x * _x))
+
+
+def _g2_fast_check(pt):
+    return _psi(pt) == F.G2.neg(_mul_int(F.G2, pt, -_x))
+
+
+def _off_subgroup_point(G, b, make_x, sqrt):
+    """the first point of y^2 = x^3 + b over x = make_x(1), make_x(2), ... outside the order-r subgroup"""
+    for k in range(1, 1000):
+        x = make_x(k)
+        if G is F.G1:
+            y = sqrt((x * x * x + b) % P_MOD)
+        else:
+            y = sqrt(F.Fp2Ops.add(F.Fp2Ops.mul(F.Fp2Ops.mul(x, x), x), b))
+        if y is not None and G.mul((x, y), R_MOD - 1) != G.neg((x, y)):
+            return (x, y)
+    raise AssertionError("no point outside the subgroup found")
+
+
+for BETA in (_w, _w * _w % P_MOD):
+    if _g1_fast_check(F.G1_GEN):
+        break
+assert pow(BETA, 3, P_MOD) == 1 and BETA != 1 and _g1_fast_check(F.G1_GEN)
+assert _g1_fast_check(F.G1.mul(F.G1_GEN, 0x1234567))
+PSI_X = F.Fp2Ops.inv(fp2_pow(XI, (P_MOD - 1) // 3))
+PSI_Y = F.Fp2Ops.inv(fp2_pow(XI, (P_MOD - 1) // 2))
+assert _g2_fast_check(F.G2_GEN) and _g2_fast_check(F.G2.mul(F.G2_GEN, 0x7654321))
+
+
+def _pairing_sqrt(a):
+    from oracle.oracle0 import pairing as _PR
+    return _PR._fp2_sqrt(a) if isinstance(a, tuple) else _PR._fp_sqrt(a)
+
+
+_bad1 = _off_subgroup_point(F.G1, F.G1_B, lambda k: k, _pairing_sqrt)
+_bad2 = _off_subgroup_point(F.G2, F.G2_B, lambda k: (k, 1), _pairing_sqrt)
+assert F.G1.is_on_curve(_bad1) and not _g1_fast_check(_bad1)
+assert F.G2.is_on_curve(_bad2) and not _g2_fast_check(_bad2)
+
 
 def emit(path, bits, ns, guard):
     n_fr, n_fp = 256 // bits, 384 // bits
@@ -130,6 +201,14 @@ def emit(path, bits, ns, guard):
                 continue                # the p^2 map is two p maps on the device; its coefficients are checked above only
             lst(name + "_C0", mont(c0, fp), n_fp)
             lst(name + "_C1", mont(c1, fp), n_fp)
+        # decode.cu: square-root exponents (plain integers), beta and the psi coefficients (Montgomery)
+        lst("EXP_SQRT", EXP_SQRT, n_fp)
+        lst("EXP_SQRT2", EXP_SQRT2, n_fp)
+        lst("BETA_M", mont(BETA, fp), n_fp)
+        lst("PSI_X_C0_M", mont(PSI_X[0], fp), n_fp)
+        lst("PSI_X_C1_M", mont(PSI_X[1], fp), n_fp)
+        lst("PSI_Y_C0_M", mont(PSI_Y[0], fp), n_fp)
+        lst("PSI_Y_C1_M", mont(PSI_Y[1], fp), n_fp)
     L.append(f"\n}}  // namespace {ns}\n")
     if macros:
         L.append("// literal limb lists: constexpr arrays are not addressable from device code")
