@@ -1,5 +1,6 @@
 // bellman_b200: C-ABI entry points that are not MSM / prover specific (include/bellman_b200.h).
 #include "bb_internal.cuh"
+#include "fixed_table.cuh"
 
 using namespace bb;
 
@@ -77,48 +78,11 @@ cudaStream_t bb_ctx::pick_stream() {
 
 namespace {
 
-// fixed-base tables for bb_fixed_base_mul: table[w*255 + d-1] = d * 2^(8w) * G, affine
-template <class F>
-struct FixedTable {
-    Affine<F>* d_table = nullptr;
-};
+// fixed-base tables of the two generators for bb_fixed_base_mul (fixed_table.cuh)
 constexpr int MAX_DEVICES = 64;
 FixedTable<Fp> g_tab1[MAX_DEVICES];      // one table per device (a process may open several contexts)
 FixedTable<Fp2> g_tab2[MAX_DEVICES];
 std::mutex g_tab_mu;
-
-template <class F>
-void batch_to_affine_host(const std::vector<XYZZ<F>>& in, std::vector<Affine<F>>& out) {
-    size_t n = in.size();
-    out.resize(n);
-    std::vector<F> pre(n);
-    F acc = FieldOps<F>::one();
-    for (size_t i = 0; i < n; i++) { pre[i] = acc; acc = acc * in[i].ZZZ; }       // no identities in the table
-    F inv = FieldOps<F>::inv(acc);
-    for (size_t i = n; i-- > 0;) {
-        F zi3 = inv * pre[i];
-        inv = inv * in[i].ZZZ;
-        F zi2 = (zi3 * in[i].ZZ).sqr();
-        out[i] = {in[i].X * zi2, in[i].Y * zi3};
-    }
-}
-
-template <class F>
-int build_fixed_table(FixedTable<F>& t, const Affine<F>& gen) {
-    if (t.d_table) return BB_OK;
-    std::vector<XYZZ<F>> pts(32 * 255);
-    XYZZ<F> base = XYZZ<F>::from_affine(gen);
-    for (int w = 0; w < 32; w++) {
-        XYZZ<F> cur = base;
-        for (int d = 1; d <= 255; d++) { pts[w * 255 + d - 1] = cur; cur.add(base); }
-        base = cur;
-    }
-    std::vector<Affine<F>> aff;
-    batch_to_affine_host(pts, aff);
-    BB_CUDA(cudaMalloc(&t.d_table, aff.size() * sizeof(Affine<F>)));
-    BB_CUDA(cudaMemcpy(t.d_table, aff.data(), aff.size() * sizeof(Affine<F>), cudaMemcpyHostToDevice));
-    return BB_OK;
-}
 
 // [k_i]G through the 32 x 255 table of byte multiples: at most 32 mixed additions per point, result left in
 // XYZZ form; zzz[i] = its ZZZ coordinate (one for the identity) for the shared inversion below

@@ -13,12 +13,34 @@
 //   k_miller             one Miller loop per pair, one thread per pair (tower.cuh)
 //   k_fp12_pair_product  the tree product of the n + 3 Miller values, one level per launch
 //   k_final_exp          final exponentiation and the comparison with one, one thread
+//
+// verify_proof for each proof of a batch (bb_groth16_verify_each; Item::verify_single, batch.rs:57-65): proof i is valid iff
+//     FE( ML(A_i, B_i) * ML(Psi_i, -gamma) * ML(C_i, -delta) ) == e(alpha, beta)^3,  Psi_i = ic[0] + sum_j x_ij ic[j+1],
+// in the device's G_T convention (tower.cuh).  Stages, one thread per proof each:
+//   k_each_psi           Psi_i by mixed additions from the byte tables of the ic points (fixed_table.cuh)
+//   k_each_miller        one multi-Miller loop over the three pairs sharing f; the two key pairs evaluate stored lines
+//   k_each_final_exp     final exponentiation, comparison with the cached target, verdict byte
+// The key data they need (EachKey) is built by the first call and cached in the bb_vk.
 #include <sys/random.h>
 
 #include "bb_internal.cuh"
+#include "fixed_table.cuh"
 #include "tower.cuh"
 
 using namespace bb;
+
+namespace {
+constexpr int MILLER_STEPS = 68;                 // 63 doubling and 5 addition steps over |x| = 0xd201000000010000
+}  // namespace
+
+// What bb_groth16_verify_each adds to bb_vk_prepare's data, built on its first call for the key
+struct EachKey {
+    Fp2* d_lines = nullptr;             // G2Prepared (lib.rs:400-409) of -gamma, then of -delta: MILLER_STEPS x (A, B, C) each
+    Fp12* d_target = nullptr;           // e(alpha, beta)^3
+    bool gamma_live = false, delta_live = false;      // false: that G2 point is the identity and its pair contributes one
+    std::vector<FixedTable<Fp>> tabs;   // tabs[j]: byte multiples of ic[j] for j >= 1; none for an identity ic[j]
+    const G1Affine** d_tabs = nullptr;  // the tables' device addresses by j (nullptr: no table)
+};
 
 struct bb_vk {
     bb_ctx* ctx = nullptr;
@@ -26,6 +48,8 @@ struct bb_vk {
     G2Affine* d_g2 = nullptr;           // delta_g2, gamma_g2, beta_g2: the G2 sides of the batch's last three pairs
     bb_bases* ic = nullptr;             // ic, resident for the Psi MSM
     size_t ic_len = 0;
+    mutable std::mutex each_mu;         // guards `each`
+    mutable EachKey* each = nullptr;
 };
 
 namespace {
@@ -324,6 +348,247 @@ int verify_batch(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* b, const vo
     return BB_OK;
 }
 
+// ---- verify_proof per proof (bb_groth16_verify_each) -----------------------------------------------------------------
+// Thread 0: the lines of -gamma (d_g2[1]), thread 1: those of -delta (d_g2[0]).  The ordinary Miller steps evaluated at
+// the unit point {x = 1, y = 1, s = 1} return the raw coefficients: they multiply A, B, C by s, x, y.
+__global__ void k_each_lines(const G2Affine* __restrict__ g2, Fp2* lines) {
+    const int t = threadIdx.x;
+    if (t > 1) return;
+    const G2Affine q = g2[t == 0 ? 1 : 0].neg();
+    if (q.is_identity()) return;
+    const Fp one = fp_one();
+    const G1Eval unit{one, one, one};
+    Fp2* out = lines + (size_t)t * MILLER_STEPS * 3;
+    G2Proj T{q.x, q.y, fp2_one()};
+    int k = 0;
+    for (int i = 62; i >= 0; i--) {
+        MillerStep d = miller_dbl_step(T, unit);
+        T = d.T;
+        out[3 * k] = d.A; out[3 * k + 1] = d.B; out[3 * k + 2] = d.C;
+        k++;
+        if ((bbc::BLS_X_ABS >> i) & 1) {
+            MillerStep a = miller_add_step(T, q, unit);
+            T = a.T;
+            out[3 * k] = a.A; out[3 * k + 1] = a.B; out[3 * k + 2] = a.C;
+            k++;
+        }
+    }
+}
+
+// e(alpha, beta)^3 with the same Miller loop and final exponentiation as every proof's value
+__global__ void k_each_target(const G1Affine* __restrict__ alpha, const G2Affine* __restrict__ g2, Fp12* target) {
+    *target = fp12_final_exp(miller_loop(g1_eval_from_affine(*alpha), g2[2]));
+}
+
+// Psi_i = ic[0] + sum_j x_ij ic[j+1] (verifier.rs:34-41): the digits of x_ij select byte multiples of ic[j+1]
+__global__ void __launch_bounds__(128) k_each_psi(const G1Affine* __restrict__ ic, const G1Affine* const* __restrict__ tabs,
+                                                  const Fr* __restrict__ x, size_t n, size_t L, G1Eval* pe) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    G1X acc = G1X::from_affine(ic[0]);
+    for (size_t j = 0; j < L; j++) {
+        const G1Affine* tab = tabs[j + 1];
+        if (!tab) continue;                                      // an identity ic[j + 1] contributes nothing
+        Fr s = fr_to_canonical(x[i * L + j]);
+        for (int w = 0; w < 32; w++) {
+            uint32_t d = (s.l[w >> 2] >> (8 * (w & 3))) & 0xffu;
+            if (d) acc.add_mixed(tab[w * 255 + d - 1]);
+        }
+    }
+    pe[i] = g1_eval_from_xyzz(acc);
+}
+
+// f * (a stored line evaluated at P): 3 Fp2 x Fp products, then the sparse product
+BB_HD Fp12 mul_stored_line(const Fp12& f, const Fp2* __restrict__ l, const G1Eval& p) {
+    return fp12_mul_line(f, fp2_mul_fp(l[0], p.s), fp2_mul_fp(l[1], p.x), fp2_mul_fp(l[2], p.y));
+}
+
+// ML(A_i, B_i) ML(Psi_i, -gamma) ML(C_i, -delta) with one f: 63 squarings in all.  f is shared, so a pair with an
+// identity on either side is skipped explicitly (its line would multiply f by zero), which gives the one that
+// multi_miller_loop gives it.
+__global__ void __launch_bounds__(MILLER_THREADS) k_each_miller(const G1Affine* __restrict__ a, const G2Affine* __restrict__ b,
+                                                                const G1Affine* __restrict__ c, const G1Eval* __restrict__ psi, size_t n,
+                                                                const Fp2* __restrict__ lines, int gamma_live, int delta_live, Fp12* f_out) {
+    size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= n) return;
+    const G1Eval pa = g1_eval_from_affine(a[idx]), pc = g1_eval_from_affine(c[idx]), pp = psi[idx];
+    const G2Affine q = b[idx];
+    const bool ab = !pa.s.is_zero() && !q.is_identity();
+    const bool pg = gamma_live && !pp.s.is_zero();
+    const bool cd = delta_live && !pc.s.is_zero();
+    const Fp2* lg = lines;
+    const Fp2* ld = lines + MILLER_STEPS * 3;
+    G2Proj T{q.x, q.y, fp2_one()};
+    Fp12 f = Fp12::one();
+    int k = 0;
+    for (int i = 62; i >= 0; i--) {
+        f = fp12_sqr(f);
+        if (ab) {
+            MillerStep d = miller_dbl_step(T, pa);
+            T = d.T;
+            f = fp12_mul_line(f, d.A, d.B, d.C);
+        }
+        if (pg) f = mul_stored_line(f, lg + 3 * k, pp);
+        if (cd) f = mul_stored_line(f, ld + 3 * k, pc);
+        k++;
+        if ((bbc::BLS_X_ABS >> i) & 1) {
+            if (ab) {
+                MillerStep s = miller_add_step(T, q, pa);
+                T = s.T;
+                f = fp12_mul_line(f, s.A, s.B, s.C);
+            }
+            if (pg) f = mul_stored_line(f, lg + 3 * k, pp);
+            if (cd) f = mul_stored_line(f, ld + 3 * k, pc);
+            k++;
+        }
+    }
+    f_out[idx] = f;
+}
+
+// Fp2 equality of the canonical values (limbs of Montgomery forms need not be unique)
+BB_HD bool fp2_equal(const Fp2& x, const Fp2& y) {
+    return fp_to_canonical(x.c0) == fp_to_canonical(y.c0) && fp_to_canonical(x.c1) == fp_to_canonical(y.c1);
+}
+BB_HD bool fp12_equal(const Fp12& x, const Fp12& y) {
+    return fp2_equal(x.c0.c0, y.c0.c0) && fp2_equal(x.c0.c1, y.c0.c1) && fp2_equal(x.c0.c2, y.c0.c2) &&
+           fp2_equal(x.c1.c0, y.c1.c0) && fp2_equal(x.c1.c1, y.c1.c1) && fp2_equal(x.c1.c2, y.c1.c2);
+}
+
+// verdict[i] = 0 if FE(f_i) == target, else 1; gt (optional) receives FE(f_i)
+__global__ void k_each_final_exp(const Fp12* __restrict__ f, size_t n, const Fp12* __restrict__ target,
+                                                                   uint8_t* verdict, Fp12* gt) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    Fp12 x = f[i];
+    Fp12 r = x.is_zero() ? x : fp12_final_exp(x);
+    if (gt) gt[i] = r;
+    verdict[i] = fp12_equal(r, *target) ? 0 : 1;
+}
+
+void each_key_free(bb_ctx* ctx, EachKey* e) {
+    for (auto& t : e->tabs)
+        if (t.d_table) cudaFree(t.d_table);
+    if (e->d_lines) ctx->release(e->d_lines);
+    if (e->d_target) ctx->release(e->d_target);
+    if (e->d_tabs) ctx->release(e->d_tabs);
+    delete e;
+}
+
+int each_key_build(bb_ctx* ctx, const bb_vk* vk, EachKey* e) {
+    const size_t m = vk->ic_len;
+    std::vector<G1Affine> ic(m);
+    G2Affine g2[3];
+    if (m) BB_CUDA(cudaMemcpy(ic.data(), vk->ic->d_points, m * sizeof(G1Affine), cudaMemcpyDeviceToHost));
+    BB_CUDA(cudaMemcpy(g2, vk->d_g2, sizeof g2, cudaMemcpyDeviceToHost));
+    e->delta_live = !g2[0].is_identity();
+    e->gamma_live = !g2[1].is_identity();
+    e->tabs.resize(m);
+    std::vector<const G1Affine*> ptrs(m > 0 ? m : 1, nullptr);
+    for (size_t j = 1; j < m; j++) {                             // ic[0] is added as it is
+        if (ic[j].is_identity()) continue;
+        BB_TRY(build_fixed_table(e->tabs[j], ic[j]));
+        ptrs[j] = e->tabs[j].d_table;
+    }
+    BB_TRY(ctx->alloc(2 * MILLER_STEPS * 3 * sizeof(Fp2), (void**)&e->d_lines));
+    BB_TRY(ctx->alloc(sizeof(Fp12), (void**)&e->d_target));
+    BB_TRY(ctx->alloc(ptrs.size() * sizeof(G1Affine*), (void**)&e->d_tabs));
+    BB_CUDA(cudaMemcpy(e->d_tabs, ptrs.data(), ptrs.size() * sizeof(G1Affine*), cudaMemcpyHostToDevice));
+    cudaStream_t st = ctx->main_stream;
+    k_each_lines<<<1, 2, 0, st>>>(vk->d_g2, e->d_lines);
+    k_each_target<<<1, 1, 0, st>>>(vk->d_alpha, vk->d_g2, e->d_target);
+    ctx->count_launch(2);
+    BB_CUDA(cudaGetLastError());
+    BB_CUDA(cudaStreamSynchronize(st));
+    return BB_OK;
+}
+
+int each_key(bb_ctx* ctx, const bb_vk* vk, const EachKey** out) {
+    std::lock_guard<std::mutex> g(vk->each_mu);
+    if (!vk->each) {
+        EachKey* e = new EachKey();
+        int s = each_key_build(ctx, vk, e);
+        if (s != BB_OK) { each_key_free(ctx, e); return s; }
+        vk->each = e;
+    }
+    *out = vk->each;
+    return BB_OK;
+}
+
+// verify_proof per proof.  gt_host: optional, n + 1 values: every proof's FE(f_i), then the target.
+int verify_each(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* b, uint8_t* verdicts, size_t* n_invalid, Fp12* gt_host) {
+    if (!ctx || !vk || !b) { set_error("bb_groth16_verify_each: null argument"); return BB_ERR_ARG; }
+    const size_t n = b->n, L = b->n_inputs;
+    if (n && (!verdicts || !n_invalid || !b->a || !b->b || !b->c || (L && !b->inputs))) {
+        set_error("bb_groth16_verify_each: null array");
+        return BB_ERR_ARG;
+    }
+    if (n && L + 1 != vk->ic_len) {                              // before any device work, as verify_batch
+        set_error("InvalidVerifyingKey: %zu public inputs for a key with %zu ic entries", L, vk->ic_len);
+        return BB_ERR_INVALID_VERIFYING_KEY;
+    }
+    if (n >= (1ull << 31)) { set_error("bb_groth16_verify_each: more than 2^31 proofs"); return BB_ERR_ARG; }
+    if (n_invalid) *n_invalid = 0;
+    if (n == 0 && !gt_host) return BB_OK;
+    BB_CUDA(cudaSetDevice(ctx->device));
+    NvtxRange nvtx("groth16_verify_each");
+    const EachKey* ek = nullptr;
+    BB_TRY(each_key(vk->ctx, vk, &ek));                         // owned by the key, like its other device buffers
+    cudaStream_t st = ctx->main_stream;
+    if (n == 0) {
+        BB_CUDA(cudaMemcpyAsync(gt_host, ek->d_target, sizeof(Fp12), cudaMemcpyDeviceToHost, st));
+        BB_CUDA(cudaStreamSynchronize(st));
+        return BB_OK;
+    }
+    StageTimer tm(ctx, st);
+    tm.mark("verify_each.begin");
+    const G1Affine *d_a = (const G1Affine*)b->a, *d_c = (const G1Affine*)b->c;
+    const G2Affine* d_b = (const G2Affine*)b->b;
+    const Fr* d_x = (const Fr*)b->inputs;
+    DevBuf up_a, up_b, up_c, up_x, d_pe, d_f, d_v, d_gt;
+    if (!b->on_device) {
+        BB_TRY(up_a.alloc(ctx, n * sizeof(G1Affine)));
+        BB_TRY(up_b.alloc(ctx, n * sizeof(G2Affine)));
+        BB_TRY(up_c.alloc(ctx, n * sizeof(G1Affine)));
+        BB_TRY(up_x.alloc(ctx, n * L * 32));
+        BB_CUDA(cudaMemcpyAsync(up_a.p, b->a, n * sizeof(G1Affine), cudaMemcpyHostToDevice, st));
+        BB_CUDA(cudaMemcpyAsync(up_b.p, b->b, n * sizeof(G2Affine), cudaMemcpyHostToDevice, st));
+        BB_CUDA(cudaMemcpyAsync(up_c.p, b->c, n * sizeof(G1Affine), cudaMemcpyHostToDevice, st));
+        if (L) BB_CUDA(cudaMemcpyAsync(up_x.p, b->inputs, n * L * 32, cudaMemcpyHostToDevice, st));
+        ctx->h2d_bytes += n * (2 * sizeof(G1Affine) + sizeof(G2Affine) + L * 32);
+        d_a = up_a.as<G1Affine>(); d_b = up_b.as<G2Affine>(); d_c = up_c.as<G1Affine>(); d_x = up_x.as<Fr>();
+    }
+    BB_TRY(d_pe.alloc(ctx, n * sizeof(G1Eval)));
+    BB_TRY(d_f.alloc(ctx, n * sizeof(Fp12)));
+    BB_TRY(d_v.alloc(ctx, n));
+    if (gt_host) BB_TRY(d_gt.alloc(ctx, n * sizeof(Fp12)));
+    tm.mark("verify_each.upload");
+    k_each_psi<<<cdiv(n, 128), 128, 0, st>>>((const G1Affine*)vk->ic->d_points, ek->d_tabs, d_x, n, L, d_pe.as<G1Eval>());
+    ctx->count_launch();
+    tm.mark("verify_each.psi");
+    k_each_miller<<<cdiv(n, MILLER_THREADS), MILLER_THREADS, 0, st>>>(d_a, d_b, d_c, d_pe.as<G1Eval>(), n, ek->d_lines, ek->gamma_live ? 1 : 0,
+                                                                      ek->delta_live ? 1 : 0, d_f.as<Fp12>());
+    ctx->count_launch();
+    tm.mark("verify_each.miller");
+    k_each_final_exp<<<cdiv(n, MILLER_THREADS), MILLER_THREADS, 0, st>>>(d_f.as<Fp12>(), n, ek->d_target, d_v.as<uint8_t>(),
+                                                                         gt_host ? d_gt.as<Fp12>() : nullptr);
+    ctx->count_launch();
+    tm.mark("verify_each.final_exp");
+    BB_CUDA(cudaGetLastError());
+    BB_CUDA(cudaMemcpyAsync(verdicts, d_v.p, n, cudaMemcpyDeviceToHost, st));
+    ctx->d2h_bytes += n;
+    if (gt_host) {
+        BB_CUDA(cudaMemcpyAsync(gt_host, d_gt.p, n * sizeof(Fp12), cudaMemcpyDeviceToHost, st));
+        BB_CUDA(cudaMemcpyAsync(gt_host + n, ek->d_target, sizeof(Fp12), cudaMemcpyDeviceToHost, st));
+    }
+    tm.mark("verify_each.download");
+    BB_CUDA(cudaStreamSynchronize(st));
+    tm.report(n);
+    size_t bad = 0;
+    for (size_t i = 0; i < n; i++) bad += verdicts[i] != 0;
+    *n_invalid = bad;
+    return BB_OK;
+}
+
 struct SplitMix {
     uint64_t s;
     uint64_t next() {
@@ -392,6 +657,7 @@ void bb_vk_destroy(bb_vk* vk) {
     if (vk->d_alpha) vk->ctx->release(vk->d_alpha);
     if (vk->d_g2) vk->ctx->release(vk->d_g2);
     if (vk->ic) bb_bases_free(vk->ic);
+    if (vk->each) each_key_free(vk->ctx, vk->each);
     delete vk;
 }
 
@@ -412,6 +678,22 @@ int bb_diag_verify_batch_gt(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* 
     int s = verify_batch(ctx, vk, batch, z, &g);
     if (s == BB_OK || s == BB_ERR_INVALID_PROOF) gt_to_canonical(g, gt_out);
     return s;
+}
+
+int bb_groth16_verify_each(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* batch, uint8_t* verdicts, size_t* n_invalid) {
+    return verify_each(ctx, vk, batch, verdicts, n_invalid, nullptr);
+}
+
+int bb_diag_verify_each_gt(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* batch, void* gt_out) {
+    if (!batch || !gt_out) { set_error("bb_diag_verify_each_gt: null argument"); return BB_ERR_ARG; }
+    const size_t n = batch->n;
+    std::vector<uint8_t> verdicts(n);
+    std::vector<Fp12> g(n + 1);
+    size_t bad = 0;
+    int s = verify_each(ctx, vk, batch, verdicts.data(), &bad, g.data());
+    if (s != BB_OK) return s;
+    for (size_t k = 0; k <= n; k++) gt_to_canonical(g[k], (uint8_t*)gt_out + k * sizeof(Fp12));
+    return BB_OK;
 }
 
 int bb_diag_multi_pairing(bb_ctx* ctx, size_t n, const void* g1, const void* g2, void* gt_out) {

@@ -5,6 +5,7 @@ bb_groth16_verify_batch.
     pvk = prepare_verifying_key(worker, vk)            # vk: the dict params_io.read_verifying_key returns
     verify_proof(pvk, (a, b, c), inputs)               # raises InvalidProof / InvalidVerifyingKey
     bv = BatchVerifier(); bv.queue(((a, b, c), inputs)); bv.verify(rng, pvk)
+    bv.verify_each(pvk)                                # verify_single per item, one device call: [None | exception, ...]
 
 Proofs are ABI-format affine point arrays (A, C: 12 u64, B: 24 u64); public inputs are Fr, either
 Python integers or an (L, 4) uint64 array in Montgomery form.
@@ -19,7 +20,7 @@ import ctypes as C
 
 import numpy as np
 
-from . import EvaluationDomain, _addr, _c64, _check, _ERRORS, _ptr, load_library
+from . import BackendError, EvaluationDomain, _addr, _c64, _check, _ERRORS, _ptr, load_library
 
 
 class VerificationError(Exception):
@@ -113,19 +114,8 @@ def verify_batch_arrays(pvk, a, b, c, inputs, z=None, on_device=False, n=None, n
     gt=True also returns the G_T value the verdict was taken from ((72,) uint64: 12 canonical Fp, tower order);
     then the verdict is returned as a bool instead of raising InvalidProof."""
     lib = load_library()
-    bt = _ProofBatch()
     keep = []
-    if on_device:
-        bt.a, bt.b, bt.c, bt.inputs = (p.value if isinstance(p, C.c_void_p) else p for p in (a, b, c, inputs))
-        bt.n, bt.n_inputs, bt.on_device = n, n_inputs, 1
-    else:
-        a, b, c = _c64(a, 12), _c64(b, 24), _c64(c, 12)
-        n = a.shape[0]
-        x = np.ascontiguousarray(inputs, dtype=np.uint64).reshape(n, -1, 4) if n else np.zeros((0, 0, 4), np.uint64)
-        L = x.shape[1] if n_inputs is None else n_inputs
-        keep += [a, b, c, x]
-        bt.a, bt.b, bt.c, bt.inputs = (arr.ctypes.data for arr in (a, b, c, x))
-        bt.n, bt.n_inputs, bt.on_device = n, L, 0
+    bt, n = _proof_batch(a, b, c, inputs, on_device, n, n_inputs, keep)
     zb = None
     if z is not None:
         assert len(z) == n
@@ -139,6 +129,43 @@ def verify_batch_arrays(pvk, a, b, c, inputs, z=None, on_device=False, n=None, n
         return False, out
     _check(rc)
     return True, out
+
+
+def _proof_batch(a, b, c, inputs, on_device, n, n_inputs, keep):
+    """the bb_proof_batch of verify_batch_arrays' arguments, and n; host arrays are appended to keep"""
+    bt = _ProofBatch()
+    if on_device:
+        bt.a, bt.b, bt.c, bt.inputs = (p.value if isinstance(p, C.c_void_p) else p for p in (a, b, c, inputs))
+        bt.n, bt.n_inputs, bt.on_device = n, n_inputs, 1
+        return bt, n
+    a, b, c = _c64(a, 12), _c64(b, 24), _c64(c, 12)
+    n = a.shape[0]
+    x = np.ascontiguousarray(inputs, dtype=np.uint64).reshape(n, -1, 4) if n else np.zeros((0, 0, 4), np.uint64)
+    L = x.shape[1] if n_inputs is None else n_inputs
+    keep += [a, b, c, x]
+    bt.a, bt.b, bt.c, bt.inputs = (arr.ctypes.data for arr in (a, b, c, x))
+    bt.n, bt.n_inputs, bt.on_device = n, L, 0
+    return bt, n
+
+
+def verify_each_arrays(pvk, a, b, c, inputs, on_device=False, n=None, n_inputs=None, gt=False):
+    """bb_groth16_verify_each: verify_proof for every proof of the arrays (arguments as for verify_batch_arrays, without z).
+    Returns the (n,) uint8 verdicts, 0 = valid, 1 = the equation fails; raises InvalidVerifyingKey for a wrong input count.
+    gt=True also returns the n + 1 G_T values ((n + 1, 72) uint64: every proof's final-exponentiated three-pair product,
+    then the key's e(alpha, beta)^k, k = gt_exponent())."""
+    lib = load_library()
+    keep = []
+    bt, n = _proof_batch(a, b, c, inputs, on_device, n, n_inputs, keep)
+    verdicts = np.zeros(max(n, 1), np.uint8)
+    n_invalid = C.c_size_t()
+    _check(lib.bb_groth16_verify_each(pvk.worker._h, pvk._h, C.byref(bt), _ptr(verdicts), C.byref(n_invalid)))
+    if n_invalid.value != int(np.count_nonzero(verdicts[:n])):
+        raise BackendError(f"bb_groth16_verify_each: n_invalid = {n_invalid.value} for {int(np.count_nonzero(verdicts[:n]))} invalid verdicts")
+    if not gt:
+        return verdicts[:n]
+    out = np.zeros((n + 1, GT_WORDS), np.uint64)
+    _check(lib.bb_diag_verify_each_gt(pvk.worker._h, pvk._h, C.byref(bt), _ptr(out)))
+    return verdicts[:n], out
 
 
 class InvalidProofEncoding(ValueError):
@@ -302,6 +329,55 @@ class BatchVerifier:
         finally:
             for p in d.values():
                 worker.device_free(p)
+
+    def verify_each(self, pvk):
+        """Item::verify_single (batch.rs:57-65) for every queued item, in one device call (bb_groth16_verify_each): the
+        fallback that finds the bad proofs of a rejected batch.  Returns one entry per item, in queue order: None, or the
+        exception verify_single would raise for it -- InvalidProof; InvalidVerifyingKey for an item with the wrong number
+        of inputs (the other items are still verified); InvalidProofEncoding (with its queue index) for a queue_bytes item
+        that does not read.  The queue_bytes items are decoded in one bb_proofs_read into device buffers and verified
+        there.  Only back-end failures raise."""
+        worker, n, L = pvk.worker, len(self.items), pvk.ic_len - 1
+        out = [None] * n
+        for i, (_, x) in enumerate(self.items):
+            if x.shape[0] != L:
+                out[i] = InvalidVerifyingKey(f"[bb_status 6] InvalidVerifyingKey: {x.shape[0]} public inputs for a key with "
+                                             f"{pvk.ic_len} ic entries (queued item {i})")
+        if n == 0 or L < 0:
+            return out
+        enc = [i for i, (p, _) in enumerate(self.items) if isinstance(p, bytes)]
+        dec = [i for i, (p, _) in enumerate(self.items) if not isinstance(p, bytes)]
+        order = enc + dec                                       # device row k holds queue item order[k]
+        x = np.zeros((n, L, 4), np.uint64)                      # zero rows for the items of a wrong input count
+        for k, i in enumerate(order):
+            if out[i] is None and L:
+                x[k] = self.items[i][1].reshape(L, 4)
+        if not enc:
+            pts = [np.stack([self.items[i][0][k].reshape(w) for i in order]) for k, w in ((0, 12), (1, 24), (2, 12))]
+            verdicts = verify_each_arrays(pvk, *pts, x, n_inputs=L)
+        else:
+            nb = len(enc)
+            d = {"a": worker.device_alloc(n * 96), "b": worker.device_alloc(n * 192), "c": worker.device_alloc(n * 96),
+                 "x": worker.device_alloc(max(1, n * L) * 32)}
+            try:
+                _, _, _, status = read_proofs(worker, b"".join(self.items[i][0] for i in enc), n=nb, out_device=(d["a"], d["b"], d["c"]))
+                for k, i in enumerate(enc):                     # Proof::read fails before the item could be queued
+                    if status[k]:
+                        out[i] = InvalidProofEncoding(f"{read_error_message(int(status[k]))} (queued proof {i})", status=int(status[k]), index=i)
+                if dec:
+                    for key, k, width in (("a", 0, 12), ("b", 1, 24), ("c", 2, 12)):
+                        rows = np.stack([self.items[i][0][k].reshape(width) for i in dec])
+                        worker.upload(C.c_void_p(_addr(d[key]) + nb * width * 8), rows)
+                if L:
+                    worker.upload(d["x"], x)
+                verdicts = verify_each_arrays(pvk, d["a"], d["b"], d["c"], d["x"], on_device=True, n=n, n_inputs=L)
+            finally:
+                for p in d.values():
+                    worker.device_free(p)
+        for k, i in enumerate(order):
+            if out[i] is None and verdicts[k]:
+                out[i] = InvalidProof(f"[bb_status 7] InvalidProof: queued item {i} does not verify")
+        return out
 
 
 def multi_pairing(worker, g1, g2):

@@ -15,8 +15,15 @@ milliseconds (CUDA events of the library's profile mode) and the Fp-multiplicati
 in pinned host memory (bb_proofs_read into HBM, then the batch verifier), the decode.* stage milliseconds and the bytes
 copied to the device per step.  Without it the line is exactly the one above.
 
+--each adds an `each` object: proofs/s of bb_groth16_verify_each (verify_proof for every proof, one device call; the
+fallback that finds the bad proofs of a rejected batch) on the same batch, in HBM and from the pinned host buffers, its
+verify_each.* stage milliseconds (from a profiled pass of their own), the Fp multiplications per proof of its kernels, the milliseconds of the key's first
+call (which builds the prepared lines and ic tables), and a check outside the timed regions: with C replaced at the first,
+middle and last index exactly those three proofs are flagged.
+
 --dump-outputs DIR writes the two verdicts and the G_T value of the rejected batch (deterministic under the seeded z)
-as float64 .npy files, the format of bench.py --dump-outputs.  Prints one JSON line on stdout; writes nothing else.
+as float64 .npy files, the format of bench.py --dump-outputs; with --each also verdicts_each, the per-proof verdicts of
+that leg's check.  Prints one JSON line on stdout; writes nothing else.
 """
 import argparse
 import importlib.util
@@ -50,6 +57,8 @@ def parse():
     ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the verdicts and the rejected batch's G_T value as DIR/<name>.npy")
     ap.add_argument("--from-bytes", action="store_true",
                     help="also time decode + verify of the batch as 192-byte Proof::write encodings in pinned host memory (adds `from_bytes`)")
+    ap.add_argument("--each", action="store_true",
+                    help="also time verify_proof for every proof of the batch in one call, bb_groth16_verify_each (adds `each`)")
     return ap.parse_args()
 
 
@@ -61,6 +70,63 @@ def miller_fp_muls_per_pair():
     dbl = 5 * 2 + 3 * 2 + 4 * 3                             # miller_dbl_step: 5 Fp2 squarings, 3 Fp2 x Fp, 4 Fp2 products
     add = 11 * 3 + 3 * 2 + 2 * 2                            # miller_add_step: 11 Fp2 products, 3 Fp2 x Fp, 2 Fp2 squarings
     return 63 * (fp12_sqr + dbl + mul_line) + 5 * (add + mul_line)
+
+
+def each_fp_muls_per_proof(n_inputs):
+    """Fp multiplications of one proof in bb_groth16_verify_each, counted as miller_fp_muls_per_pair counts them (an Fp2
+    product 3, an Fp2 squaring or Fp2 x Fp product 2; inversions by fp_inv_gcd not counted)"""
+    fp12_sqr, mul_line, dbl, add = 36, 45, 28, 43
+    stored_line = 3 * 2 + mul_line                          # a stored line at P: 3 Fp2 x Fp products, then the sparse product
+    psi = n_inputs * 32 * 10 + 3                            # k_each_psi: mixed XYZZ additions (8 products, 2 squarings), G1Eval
+    miller = 63 * (fp12_sqr + dbl + mul_line + 2 * stored_line) + 5 * (add + mul_line + 2 * stored_line)
+    fp12_mul, cyc_sqr, frob1, frob2, inv = 54, 18, 15, 30, 109
+    exp_x = 63 * cyc_sqr + 5 * fp12_mul
+    final_exp = (inv + fp12_mul + frob2 + fp12_mul                                  # easy part
+                 + 5 * exp_x + 2 * fp12_mul + fp12_mul + frob1                        # five x-powers; (x - 1)^2; x + p
+                 + 2 * fp12_mul + frob2 + 2 * fp12_mul + cyc_sqr                      # x^2 + p^2 - 1; t^3
+                 + 24)                                                                # the canonical comparison
+    return {"psi": psi, "miller": miller, "final_exp": final_exp, "total": psi + miller + final_exp}
+
+
+EACH_STAGES = ("upload", "psi", "miller", "final_exp", "download")
+
+
+def each_leg(args, worker, pvk, d, host, timed):
+    """--each: bb_groth16_verify_each on the timed batch, from HBM and from the pinned host buffers.  Outside the timed
+    regions: the key's first call (it builds the prepared lines and ic tables), and C replaced at the first, middle and
+    last index, which must flag exactly those three."""
+    from bellman_b200 import verifier as V
+    n, L = host["a"].shape[0], args.inputs
+    t0 = time.perf_counter()
+    first = V.verify_each_arrays(pvk, d["a"], d["b"], d["c"], d["x"], on_device=True, n=n, n_inputs=L)
+    first_ms = 1e3 * (time.perf_counter() - t0)
+
+    def step_value():
+        V.verify_each_arrays(pvk, d["a"], d["b"], d["c"], d["x"], on_device=True, n=n, n_inputs=L)
+
+    def step_e2e():
+        V.verify_each_arrays(pvk, host["a"], host["b"], host["c"], host["x"], n_inputs=L)
+
+    dt, launches, _ = timed(step_value)
+    dt_e2e, _, h2d = timed(step_e2e)
+    worker.set_option("profile", 1)                         # the stages in a run of their own: the timings above are unprofiled
+    timed(step_value)
+    stages = {s: worker.profile_read("verify_each." + s)[0] / args.steps for s in EACH_STAGES}
+    worker.set_option("profile", 0)
+    bad = sorted({0, n // 2, n - 1})
+    c_bad = host["c"].copy()
+    for pos in bad:
+        c_bad[pos] = host["c"][(pos + 1) % n]
+    verdicts = V.verify_each_arrays(pvk, host["a"], host["b"], c_bad, host["x"], n_inputs=L)     # n_invalid is checked there
+    flagged = np.flatnonzero(verdicts).tolist()
+    checks = {"flagged": "first, middle, last" if flagged == bad and not first.any() else f"{flagged} (timed batch: {np.flatnonzero(first).tolist()})",
+              "n_invalid": int(np.count_nonzero(verdicts))}
+    return {"value": n * args.steps / dt, "unit": "proofs/s", "ms_per_step": 1e3 * dt / args.steps, "gpu_launches": int(launches),
+            "e2e": {"value": n * args.steps / dt_e2e, "unit": "proofs/s", "ms_per_step": 1e3 * dt_e2e / args.steps, "h2d_bytes_per_step": int(h2d)},
+            "stages_ms_per_step": {k: round(v, 3) for k, v in stages.items()},
+            "fp_mul_per_proof": each_fp_muls_per_proof(L), "first_call_ms": round(first_ms, 3),
+            "source": "the timed batch; step = bb_groth16_verify_each (verdicts for every proof, no z)",
+            "checks": checks}, verdicts
 
 
 DECODE_STAGES = ("decode.upload", "decode.g1", "decode.g2", "decode.status", "decode.download")
@@ -184,6 +250,7 @@ def run(args):
     ok_bad, gt_bad = V.verify_batch_arrays(pvk, host["a"], host["b"], c_bad, host["x"], z=z, n_inputs=L, gt=True)
     checks = {"timed_batch": "accepted" if ok else "REJECTED", "one_c_replaced": "rejected" if not ok_bad else "ACCEPTED"}
     from_bytes = from_bytes_leg(args, worker, pvk, d, host, z, timed) if args.from_bytes else None
+    each, verdicts_each = each_leg(args, worker, pvk, d, host, timed) if args.each else (None, None)
     per_pair = miller_fp_muls_per_pair()
     miller_ms = stages["miller"]
     line = {"metric": "groth16_batch_verify_proofs_per_sec", "value": n * args.steps / dt_val, "unit": "proofs/s", "n_gpus": 1,
@@ -206,11 +273,18 @@ def run(args):
             "cpu_baseline_reason": "oracle-1 has no CPU pairing; the Python pairing of oracle-0 is a correctness reference, not a timed baseline"}
     if from_bytes is not None:
         line["from_bytes"] = from_bytes
-    bench.dump_outputs(args.dump_outputs, {"verdicts": np.array([int(ok), int(ok_bad)], np.uint32), "gt_tampered": gt_bad})
+    if each is not None:
+        line["each"] = each
+    dumps = {"verdicts": np.array([int(ok), int(ok_bad)], np.uint32), "gt_tampered": gt_bad}
+    if each is not None:
+        dumps["verdicts_each"] = verdicts_each
+    bench.dump_outputs(args.dump_outputs, dumps)
     bench.emit(line)
     assert ok and not ok_bad, checks
     if from_bytes is not None:
         assert from_bytes["checks"] == {"decoded_points": "equal", "corrupted_b_at_middle": "reported"}, from_bytes["checks"]
+    if each is not None:
+        assert each["checks"] == {"flagged": "first, middle, last", "n_invalid": 3}, each["checks"]
     pvk.free()
     for p in d.values():
         worker.device_free(p)

@@ -298,6 +298,15 @@ int bb_groth16_verify(bb_ctx* ctx, const bb_vk* vk, const void* a, const void* b
  * z: n canonical 32-byte scalars in [1, r) (zero or >= r: BB_ERR_ARG), or NULL = drawn from the operating system
  * (getrandom, zeros redrawn).  The key check comes first, before any device work.  An empty batch is accepted. */
 int bb_groth16_verify_batch(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* batch, const void* z);
+/* Item::verify_single (batch.rs:57-65), i.e. verify_proof (verifier.rs:23-58), for each of the n proofs of `batch`
+ * (bb_proof_batch as for bb_groth16_verify_batch; host or device buffers): the fallback that finds the invalid proofs of
+ * a rejected batch, in one call.  Deterministic (no z).  verdicts: n bytes, host, always written: 0 = valid, 1 = the
+ * equation fails.  *n_invalid = number of non-zero verdicts.  BB_OK whenever the call ran, even if some proofs are invalid
+ * (as bb_proofs_read).  BB_ERR_INVALID_VERIFYING_KEY: n > 0 and n_inputs + 1 != ic_len, before any device work.
+ * BB_ERR_ARG: NULL pointers with n > 0, n >= 2^31.  An empty batch is BB_OK.  The first call for a key builds and keeps
+ * with it the prepared lines of -gamma and -delta, e(alpha, beta) and a 784 KB table of byte multiples per non-identity
+ * ic[j], j >= 1 (freed by bb_vk_destroy). */
+int bb_groth16_verify_each(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* batch, uint8_t* verdicts, size_t* n_invalid);
 
 /* ---- reading and writing proofs: Proof::read / Proof::write (groth16/src/lib.rs:39-99) -------------------------
  * A proof is 192 bytes: compressed A (48 B), B (96 B), C (48 B), the ZCash encoding of bls12_381 0.8.  Decoding runs

@@ -54,6 +54,9 @@ int bb_diag_gt_exponent(void);
 int bb_diag_fp12(bb_ctx* ctx, int op, const void* a, const void* b, void* out, size_t n);
 /* bb_groth16_verify_batch, also writing the G_T value its verdict was taken from (format of bb_diag_multi_pairing) */
 int bb_diag_verify_batch_gt(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* batch, const void* z, void* gt_out);
+/* bb_groth16_verify_each, writing n + 1 G_T values (format of bb_diag_multi_pairing): for each proof the final-exponentiated
+ * ML(A_i, B_i) ML(Psi_i, -gamma) ML(C_i, -delta), then the key's e(alpha, beta)^3 they are compared with */
+int bb_diag_verify_each_gt(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* batch, void* gt_out);
 /* a synthetic verifying key and n valid proofs from trapdoor scalars drawn from `seed`:
  * alpha, beta, gamma, delta, ic_j = [t_j] G1 (j <= n_inputs); proof i: A = [a_i] G1, B = [b_i] G2,
  * C = [(a_i b_i - alpha beta - gamma sum_j x_ij t_j) / delta] G1 (x_i0 = 1), all by fixed-base multiplication on the device.

@@ -159,6 +159,8 @@ extern "C" {
     pub fn bb_groth16_verify(ctx: *mut bb_ctx, vk: *const bb_vk, a: *const c_void, b: *const c_void, c: *const c_void,
                              inputs: *const c_void, n_inputs: usize) -> c_int;
     pub fn bb_groth16_verify_batch(ctx: *mut bb_ctx, vk: *const bb_vk, batch: *const bb_proof_batch, z: *const c_void) -> c_int;
+    pub fn bb_groth16_verify_each(ctx: *mut bb_ctx, vk: *const bb_vk, batch: *const bb_proof_batch, verdicts: *mut u8,
+                                  n_invalid: *mut usize) -> c_int;
     pub fn bb_proofs_read(ctx: *mut bb_ctx, input: *const bb_proof_bytes, a: *mut c_void, b: *mut c_void, c: *mut c_void,
                           out_on_device: c_int, status: *mut u8, n_invalid: *mut usize) -> c_int;
     pub fn bb_proofs_write(ctx: *mut bb_ctx, a: *const c_void, b: *const c_void, c: *const c_void, n: usize, on_device: c_int,

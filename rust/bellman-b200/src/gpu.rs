@@ -241,7 +241,7 @@ pub fn create_proof_b200(w: &WitnessView, crs: &GpuParameters, r: Scalar, s: Sca
 }
 
 /// `PreparedVerifyingKey` (groth16/src/lib.rs:400-409, verifier.rs:11-21): the verifying key resident on the device.
-pub struct GpuVerifyingKey { pub(crate) ctx: *mut bb_ctx, pub(crate) handle: *mut bb_vk }
+pub struct GpuVerifyingKey { pub(crate) ctx: *mut bb_ctx, pub(crate) handle: *mut bb_vk, pub(crate) ic_len: usize }
 unsafe impl Send for GpuVerifyingKey {}
 unsafe impl Sync for GpuVerifyingKey {}
 
@@ -272,7 +272,7 @@ impl GpuVerifyingKey {
         };
         let mut handle = ptr::null_mut();
         status(unsafe { bb_vk_prepare(worker.ctx, &desc, &mut handle) })?;
-        Ok(GpuVerifyingKey { ctx: worker.ctx, handle })
+        Ok(GpuVerifyingKey { ctx: worker.ctx, handle, ic_len: vk.ic.len() })
     }
 }
 impl Drop for GpuVerifyingKey {
@@ -404,6 +404,93 @@ pub fn batch_verify_bytes_b200<R: RngCore + CryptoRng>(worker: &GpuWorker, vk: &
     let batch = bb_proof_batch { a: d_a.p, b: d_b.p, c: d_c.p, n, inputs: d_x.p, n_inputs, on_device: 1 };
     verification_status(unsafe { bb_groth16_verify_batch(worker.ctx, vk.handle, &batch, z.as_ptr() as _) })
         .map_err(BytesBatchError::Verification)
+}
+
+/// verify_single's key check for one item (batch.rs:57-65 -> verifier.rs:28-30)
+fn input_count(pvk: &GpuVerifyingKey, x: &[Scalar]) -> Result<(), VerificationError> {
+    if x.len() + 1 == pvk.ic_len { Ok(()) } else { Err(VerificationError::InvalidVerifyingKey) }
+}
+
+/// The n x L input matrix of the items, with zero rows for the items of a wrong input count (their verdicts are not used).
+fn each_inputs<'a>(pvk: &GpuVerifyingKey, xs: impl Iterator<Item = &'a Vec<Scalar>>, n: usize) -> Vec<Scalar> {
+    let l = pvk.ic_len - 1;
+    let mut inputs = vec![Scalar::from(0u64); n * l];
+    for (i, x) in xs.enumerate() {
+        if x.len() == l { inputs[i * l..(i + 1) * l].copy_from_slice(x); }
+    }
+    inputs
+}
+
+/// bb_groth16_verify_each: one verdict byte per proof of the batch, 0 = valid
+fn each_verdicts(pvk: &GpuVerifyingKey, batch: &bb_proof_batch) -> Vec<u8> {
+    let mut verdicts = vec![0u8; batch.n];
+    let mut n_invalid = 0usize;
+    let rc = unsafe { bb_groth16_verify_each(pvk.ctx, pvk.handle, batch, verdicts.as_mut_ptr(), &mut n_invalid) };
+    if rc != BB_OK { panic!("bellman_b200 bb_groth16_verify_each failed: {}", last_error()); }
+    verdicts
+}
+
+/// `Item::verify_single` (verifier/batch.rs:57-65), i.e. `verify_proof`, for every item in one device call: the fallback
+/// that finds the bad proofs of a batch `batch_verify_b200` rejected.  One result per item, in order: InvalidVerifyingKey
+/// for an item whose input count does not match the key (the other items are still verified), InvalidProof for an item
+/// whose equation fails.
+pub fn verify_each_b200(pvk: &GpuVerifyingKey, items: &[(Proof<Bls12>, Vec<Scalar>)]) -> Vec<Result<(), VerificationError>> {
+    let n = items.len();
+    let mut out: Vec<Result<(), VerificationError>> = items.iter().map(|(_, x)| input_count(pvk, x)).collect();
+    if n == 0 || pvk.ic_len == 0 { return out; }
+    let (mut a, mut b, mut c) = (Vec::with_capacity(n * 12), Vec::with_capacity(n * 24), Vec::with_capacity(n * 12));
+    for (proof, _) in items {
+        a.extend(flat(&[proof.a]));
+        b.extend(flat(&[proof.b]));
+        c.extend(flat(&[proof.c]));
+    }
+    let inputs = each_inputs(pvk, items.iter().map(|(_, x)| x), n);
+    let batch = bb_proof_batch {
+        a: a.as_ptr() as _, b: b.as_ptr() as _, c: c.as_ptr() as _, n,
+        inputs: inputs.as_ptr() as _, n_inputs: pvk.ic_len - 1, on_device: 0,
+    };
+    for (r, v) in out.iter_mut().zip(each_verdicts(pvk, &batch)) {
+        if r.is_ok() && v != 0 { *r = Err(VerificationError::InvalidProof); }
+    }
+    out
+}
+
+/// `verify_each_b200` over items given as `Proof::write` bytes: one bb_proofs_read decodes every proof into device buffers
+/// and bb_groth16_verify_each runs on them there.  One result per item, in order: `Read` (its index and the io::Error of
+/// `Proof::read`; a shorter item fails as `read_exact` does) for a proof that does not read, otherwise what
+/// `verify_each_b200` gives for it.
+pub fn verify_each_bytes_b200(worker: &GpuWorker, pvk: &GpuVerifyingKey, items: &[(&[u8], Vec<Scalar>)]) -> Vec<Result<(), BytesBatchError>> {
+    let n = items.len();
+    let mut bytes = Vec::with_capacity(n * BB_PROOF_BYTES);
+    for (b, _) in items {
+        if b.len() < BB_PROOF_BYTES { bytes.extend_from_slice(&[0u8; BB_PROOF_BYTES]); } else { bytes.extend_from_slice(&b[..BB_PROOF_BYTES]); }
+    }
+    let (d_a, d_b, d_c) = (DeviceBuf::new(worker.ctx, n * 96), DeviceBuf::new(worker.ctx, n * 192), DeviceBuf::new(worker.ctx, n * 96));
+    let mut st = vec![0u8; n];
+    let mut n_invalid = 0usize;
+    let input = bb_proof_bytes { bytes: bytes.as_ptr() as _, n, stride: BB_PROOF_BYTES, on_device: 0 };
+    let rc = unsafe { bb_proofs_read(worker.ctx, &input, d_a.p, d_b.p, d_c.p, 1, st.as_mut_ptr(), &mut n_invalid) };
+    if rc != BB_OK { panic!("bellman_b200 bb_proofs_read failed: {}", last_error()); }
+    let mut out: Vec<Result<(), BytesBatchError>> = items.iter().enumerate().map(|(index, (b, x))| {
+        if b.len() < BB_PROOF_BYTES {
+            Err(BytesBatchError::Read { index, error: io::Error::new(io::ErrorKind::UnexpectedEof, "failed to fill whole buffer") })
+        } else if st[index] != 0 {
+            Err(BytesBatchError::Read { index, error: read_error(st[index]) })
+        } else {
+            input_count(pvk, x).map_err(BytesBatchError::Verification)
+        }
+    }).collect();
+    if n == 0 || pvk.ic_len == 0 { return out; }
+    let inputs = each_inputs(pvk, items.iter().map(|(_, x)| x), n);
+    let d_x = DeviceBuf::new(worker.ctx, inputs.len() * 32);
+    if !inputs.is_empty() && unsafe { bb_device_upload(worker.ctx, d_x.p, inputs.as_ptr() as _, inputs.len() * 32) } != BB_OK {
+        panic!("bellman_b200 upload failed: {}", last_error());
+    }
+    let batch = bb_proof_batch { a: d_a.p, b: d_b.p, c: d_c.p, n, inputs: d_x.p, n_inputs: pvk.ic_len - 1, on_device: 1 };
+    for (r, v) in out.iter_mut().zip(each_verdicts(pvk, &batch)) {
+        if r.is_ok() && v != 0 { *r = Err(BytesBatchError::Verification(VerificationError::InvalidProof)); }
+    }
+    out
 }
 
 #[allow(dead_code)]
