@@ -158,16 +158,13 @@ struct PairLoader {
 template <class F>
 __device__ __forceinline__ F ld_field(const F* p) { return ldg_words(p); }
 
-// resident CTAs per SM the phase kernels are compiled for (0 = whatever the registers allow).  G1 fits four
-// CTAs of 128 threads at 126-128 registers by itself; BB_AFF_G2_MINB caps the Fp2 instantiations (204
-// registers, two CTAs) for A/B runs.
-#ifndef BB_AFF_G2_MINB
-#define BB_AFF_G2_MINB 1
-#endif
-template <class F> struct AffBounds { static constexpr int MINB = 1; };
-template <> struct AffBounds<Fp2> { static constexpr int MINB = BB_AFF_G2_MINB; };
+// minimum resident CTAs of 128 threads per SM for phase 3 (ptxas -v, sm_90a, see DESIGN 4.1).  G1 needs ~176
+// registers unbounded (two CTAs); three CTAs cap it at 168, which it fits without spilling.  G2 takes all 255.
+template <class F> struct AffBounds { static constexpr int MINB = 3; };
+template <> struct AffBounds<Fp2> { static constexpr int MINB = 1; };
 
-// phase 1: denominators and their running products
+// phase 1: denominators and their running products.  The products are inlined (FieldOps): an out-of-line Fp2
+// product would keep its operands in a local-memory stack frame.
 template <class F, bool GATHER>
 __global__ void __launch_bounds__(128) k_aff_phase1(PairLoader<F, GATHER> ld, const uint32_t* __restrict__ d_entries, uint32_t shift,
                                                     size_t T, uint32_t L, F* __restrict__ pre, F* __restrict__ tp) {
@@ -195,18 +192,53 @@ __global__ void __launch_bounds__(128) k_aff_phase1(PairLoader<F, GATHER> ld, co
             }
         }
         st_words(pre + j, run);
-        run = run * den;
+        run = FieldOps<F>::mul(run, den);
     }
     st_words(tp + t, run);
 }
 
+// Operands of pair j for phase 3.  Returns false when the sum needs no inversion; it has then been written to
+// out[j] already: the other operand for a null / identity one, the identity for P + (-P).  Otherwise *den / *num
+// are the slope's denominator and numerator, and x1, x2, y1 what the sum needs of the operands.  Each operand is
+// stored separately (no `i1 ? P2 : P1`: selecting between two local points by reference put both in a stack frame).
+// err[1] is raised for an identity base selected by a digit (Source::next, multiexp.rs:63-65): only gathered rows
+// can be CRS bases.
+template <class F, bool GATHER>
+__device__ __forceinline__ bool pair_operands(const PairLoader<F, GATHER>& ld, size_t j, Affine<F>* __restrict__ out, uint32_t* err,
+                                              F* den, F* num, F* x1, F* x2, F* y1) {
+    bool n1, n2, g1, g2;
+    const Affine<F>* r1 = ld.row(j, 0, &n1, &g1);
+    const Affine<F>* r2 = ld.row(j, 1, &n2, &g2);
+    Affine<F> P1 = n1 ? Affine<F>::identity() : ld_affine(r1);
+    Affine<F> P2 = n2 ? Affine<F>::identity() : ld_affine(r2);
+    const bool i1 = affine_is_identity(P1), i2 = affine_is_identity(P2);
+    if (GATHER && ((i1 && !n1) || (i2 && !n2))) atomicOr(&err[1], 1u);
+    if (g1) P1.y = P1.y.neg();
+    if (g2) P2.y = P2.y.neg();
+    if (i1) { st_words(out + j, P2); return false; }
+    if (i2) { st_words(out + j, P1); return false; }
+    *den = P2.x - P1.x;
+    if (den->is_zero()) {
+        if (P1.y != P2.y || P1.y.is_zero()) { st_words(out + j, Affine<F>::identity()); return false; }
+        *den = P1.y.dbl();
+        F xx = FieldOps<F>::sqr(P1.x);
+        *num = xx.dbl() + xx;
+    } else {
+        *num = P2.y - P1.y;
+    }
+    *x1 = P1.x;
+    *x2 = P2.x;
+    *y1 = P1.y;
+    return true;
+}
+
 // phase 3: finish the additions, walking the thread's pairs backwards.  tp[t] = 1 / (product of the
-// thread's denominators).  err[1] is raised for an identity base selected by a digit (Source::next,
-// multiexp.rs:63-65) -- only gathered rows can be CRS bases.
+// thread's denominators).  Products inlined as in phase 1.
 template <class F, bool GATHER>
 __global__ void __launch_bounds__(128, AffBounds<F>::MINB) k_aff_phase3(PairLoader<F, GATHER> ld, const uint32_t* __restrict__ d_entries, uint32_t shift,
-                                                    size_t T, uint32_t L, const F* __restrict__ pre, const F* __restrict__ tp,
-                                                    Affine<F>* __restrict__ out, uint32_t* err) {
+                                                                        size_t T, uint32_t L, const F* __restrict__ pre, const F* __restrict__ tp,
+                                                                        Affine<F>* __restrict__ out, uint32_t* err) {
+    typedef FieldOps<F> O;
     size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= T) return;
     const size_t npairs = (size_t)(*d_entries) >> shift;
@@ -216,31 +248,14 @@ __global__ void __launch_bounds__(128, AffBounds<F>::MINB) k_aff_phase3(PairLoad
     if (cnt > L) cnt = L;
     for (int i = (int)cnt - 1; i >= 0; i--) {
         size_t j = (size_t)i * T + t;
-        bool n1, n2, g1, g2;
-        const Affine<F>* r1 = ld.row(j, 0, &n1, &g1);
-        const Affine<F>* r2 = ld.row(j, 1, &n2, &g2);
-        Affine<F> P1 = n1 ? Affine<F>::identity() : ld_affine(r1);
-        Affine<F> P2 = n2 ? Affine<F>::identity() : ld_affine(r2);
-        bool i1 = affine_is_identity(P1), i2 = affine_is_identity(P2);
-        if (GATHER && ((i1 && !n1) || (i2 && !n2))) atomicOr(&err[1], 1u);
-        if (g1) P1.y = P1.y.neg();
-        if (g2) P2.y = P2.y.neg();
-        if (i1 || i2) { st_words(out + j, i1 ? P2 : P1); continue; }
-        F den = P2.x - P1.x, num;
-        if (den.is_zero()) {
-            if (P1.y != P2.y || P1.y.is_zero()) { st_words(out + j, Affine<F>::identity()); continue; }
-            den = P1.y.dbl();
-            F xx = P1.x.sqr();
-            num = xx.dbl() + xx;
-        } else {
-            num = P2.y - P1.y;
-        }
-        F inv = run * ld_words(pre + j);
-        run = run * den;
-        F lam = num * inv;
+        F den, num, x1, x2, y1;
+        if (!pair_operands(ld, j, out, err, &den, &num, &x1, &x2, &y1)) continue;
+        F inv = O::mul(run, ld_words(pre + j));
+        run = O::mul(run, den);
+        F lam = O::mul(num, inv);
         Affine<F> R;
-        R.x = lam.sqr() - P1.x - P2.x;
-        R.y = lam * (P1.x - R.x) - P1.y;
+        R.x = O::sqr(lam) - x1 - x2;
+        R.y = O::mul(lam, x1 - R.x) - y1;
         st_words(out + j, R);
     }
 }

@@ -123,7 +123,12 @@ struct Fp2 {
     BB_HD bool operator!=(const Fp2& o) const { return !(*this == o); }
     BB_HD Fp2 operator+(const Fp2& o) const { return {c0 + o.c0, c1 + o.c1}; }
     BB_HD Fp2 operator-(const Fp2& o) const { return {c0 - o.c0, c1 - o.c1}; }
-    BB_HD_NOINLINE Fp2 operator*(const Fp2& o) const { // Karatsuba: 3 Fp products
+    // Out of line on the device (BB_HD_NOINLINE): the tower, verifier and reduction kernels make hundreds of these
+    // calls.  The operands of such a call are passed by address, so the caller keeps them in its local-memory stack
+    // frame; the halving-round kernels (batch_affine.cuh) use the inlined forms through FieldOps instead.
+    BB_HD_NOINLINE Fp2 operator*(const Fp2& o) const { return mul_inl(o); }
+    BB_HD_NOINLINE Fp2 sqr() const { return sqr_inl(); }
+    BB_HD Fp2 mul_inl(const Fp2& o) const {              // Karatsuba: 3 Fp products
 #if defined(BB_DEVPATH) && BB_FP2_LAZY
         // lazy reduction: three 24-limb integer products, two Montgomery reductions.
         //   c0 = redc(a0 b0 + p^2 - a1 b1)              (< 2 p^2)
@@ -162,7 +167,7 @@ struct Fp2 {
         return {aa - bb_, t - aa - bb_};
 #endif
     }
-    BB_HD_NOINLINE Fp2 sqr() const {                   // (c0+c1)(c0-c1), 2 c0 c1
+    BB_HD Fp2 sqr_inl() const {                        // (c0+c1)(c0-c1), 2 c0 c1
         Fp s = c0 + c1, d = c0 - c1, m = c0 * c1;
         return {s * d, m + m};
     }
@@ -178,16 +183,20 @@ BB_HD Fp2 fp2_inv(const Fp2& a) {
     return {a.c0 * n, (a.c1 * n).neg()};
 }
 
-// uniform field-trait view used by the curve templates
+// uniform field-trait view used by the curve templates; mul / sqr are always inlined
 template <class F> struct FieldOps;
 template <> struct FieldOps<Fp> {
     BB_HD static Fp one() { return fp_one(); }
     BB_HD static Fp inv(const Fp& a) { return fp_inv_gcd(a); }
+    BB_HD static Fp mul(const Fp& a, const Fp& b) { return a * b; }
+    BB_HD static Fp sqr(const Fp& a) { return a.sqr(); }
     static constexpr int WORDS = 12;
 };
 template <> struct FieldOps<Fp2> {
     BB_HD static Fp2 one() { return fp2_one(); }
     BB_HD static Fp2 inv(const Fp2& a) { return fp2_inv(a); }
+    BB_HD static Fp2 mul(const Fp2& a, const Fp2& b) { return a.mul_inl(b); }
+    BB_HD static Fp2 sqr(const Fp2& a) { return a.sqr_inl(); }
     static constexpr int WORDS = 24;
 };
 
