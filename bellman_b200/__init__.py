@@ -680,3 +680,5 @@ from .verifier import (BatchVerifier, InvalidProof, InvalidVerifyingKey, Prepare
                        VerificationError, prepare_verifying_key, verify_proof)
 # Proof::read / Proof::write over a batch (groth16/src/lib.rs:39-99)
 from .verifier import InvalidProofEncoding, read_proof, read_proofs, write_proofs  # noqa: E402
+# the constraint system on the device: prove from the witness alone (groth16/src/prover.rs:19-55,105-145)
+from .r1cs import R1CS, create_proof_r1cs, create_random_proof_r1cs  # noqa: E402

@@ -1,0 +1,355 @@
+// bellman_b200: the constraint system resident on the device.  ProvingAssignment::enforce
+// (bellman/groth16/src/prover.rs:105-145) evaluates every linear combination of every constraint
+// on the caller's CPU, one field product per term, inside synthesis.  Nothing in that work depends
+// on anything but the circuit's shape and the witness, so the handle here keeps the A, B and C
+// matrices in HBM beside the key and computes a = A z, b = B z, c = C z as a sparse
+// matrix-vector product over Fr, with z = input_assignment || aux_assignment.
+//
+// Layout (built on the host at create time, DESIGN.md 4.8):
+//   the three matrices as ONE CSR of 3 N rows (N = constraints incl. the appended input rows;
+//   row g = matrix g / N, constraint g % N), uint32 offsets;
+//   per term a uint32 variable index (inputs first, then aux) whose bit 31 marks coefficient one
+//   (eval skips that product, prover.rs:47-49), and its Fr coefficient (Montgomery) at the same
+//   position; terms with coefficient zero are dropped (they add nothing, and the densities are
+//   taken before);
+//   the row ids binned by length: <= 32 terms one thread per row, 33..2048 one warp per row,
+//   more one CTA of 256 threads per row.
+#include <memory>
+#include <vector>
+
+#include "bb_internal.cuh"
+
+using namespace bb;
+
+namespace {
+
+constexpr uint32_t ONE_FLAG = 0x80000000u;
+constexpr uint32_t SHORT_MAX = 32;     // terms: one thread per row up to here
+constexpr uint32_t WARP_MAX = 2048;    // one warp per row up to here, one CTA above
+constexpr int GROUP_THREADS = 256;
+
+struct EvalArgs {
+    const uint32_t* off;
+    const uint32_t* idx;
+    const Fr* coef;
+    const Fr* input;
+    const Fr* aux;
+    Fr *out_a, *out_b, *out_c;
+    uint32_t n_inputs;
+    uint32_t n;                        // rows per matrix
+};
+
+__device__ __forceinline__ Fr r1cs_term(const EvalArgs& A, uint32_t k) {
+    const uint32_t v = A.idx[k], var = v & ~ONE_FLAG;
+    const Fr z = var < A.n_inputs ? A.input[var] : A.aux[var - A.n_inputs];
+    return (v & ONE_FLAG) ? z : A.coef[k] * z;
+}
+
+__device__ __forceinline__ void r1cs_put(const EvalArgs& A, uint32_t g, const Fr& v) {
+    Fr* o = g < A.n ? A.out_a : g < 2 * A.n ? A.out_b : A.out_c;
+    o[g - (g < A.n ? 0 : g < 2 * A.n ? A.n : 2 * A.n)] = v;
+}
+
+// rows of at most SHORT_MAX terms (MiMC-like rows of 1-3 terms, empty rows): one thread each
+__global__ void __launch_bounds__(128) k_r1cs_rows_thread(EvalArgs A, const uint32_t* __restrict__ rows, uint32_t count) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    const uint32_t g = rows[i];
+    Fr acc = Fr::zero();
+    for (uint32_t k = A.off[g], e = A.off[g + 1]; k < e; k++) acc = acc + r1cs_term(A, k);
+    r1cs_put(A, g, acc);
+}
+
+// long rows: GROUP threads per row stride over its terms, then a tree of Fr additions in shared memory
+template <int GROUP>
+__global__ void __launch_bounds__(GROUP_THREADS) k_r1cs_rows_group(EvalArgs A, const uint32_t* __restrict__ rows, uint32_t count) {
+    __shared__ Fr sh[GROUP_THREADS];
+    const uint32_t lane = threadIdx.x % GROUP, slot = blockIdx.x * (GROUP_THREADS / GROUP) + threadIdx.x / GROUP;
+    Fr acc = Fr::zero();
+    uint32_t g = 0;
+    if (slot < count) {
+        g = rows[slot];
+        for (uint32_t k = A.off[g] + lane, e = A.off[g + 1]; k < e; k += GROUP) acc = acc + r1cs_term(A, k);
+    }
+    sh[threadIdx.x] = acc;
+    __syncthreads();
+    for (uint32_t s = GROUP / 2; s > 0; s >>= 1) {
+        if (lane < s) sh[threadIdx.x] = sh[threadIdx.x] + sh[threadIdx.x + s];
+        __syncthreads();
+    }
+    if (lane == 0 && slot < count) r1cs_put(A, g, sh[threadIdx.x]);
+}
+
+bool fr_geq_modulus(const uint32_t* v) {
+    for (int i = 7; i >= 0; i--) {
+        if (v[i] > bbc::FR_MOD[i]) return true;
+        if (v[i] < bbc::FR_MOD[i]) return false;
+    }
+    return true;
+}
+
+// CUDA-event brackets of the stages (profile mode only), as in decode.cu
+struct R1csTimer {
+    bb_ctx* ctx;
+    cudaStream_t st;
+    std::vector<std::pair<const char*, cudaEvent_t>> marks;
+    R1csTimer(bb_ctx* c, cudaStream_t s) : ctx(c), st(s) {}
+    ~R1csTimer() { for (auto& m : marks) cudaEventDestroy(m.second); }
+    void mark(const char* stage_ending_here) {
+        if (!ctx->opt_profile) return;
+        cudaEvent_t e;
+        if (cudaEventCreate(&e) != cudaSuccess) return;
+        cudaEventRecord(e, st);
+        marks.emplace_back(stage_ending_here, e);
+    }
+    void report(uint64_t units) {
+        for (size_t k = 1; k < marks.size(); k++) {
+            float ms = 0;
+            if (cudaEventElapsedTime(&ms, marks[k - 1].second, marks[k].second) == cudaSuccess) ctx->prof_add(marks[k].first, ms, 1, units);
+        }
+    }
+};
+
+}  // namespace
+
+struct bb_r1cs {
+    bb_ctx* ctx = nullptr;
+    size_t n_inputs = 0, n_aux = 0, n = 0;              // n: constraints including the appended input rows
+    uint64_t nnz[3] = {0, 0, 0}, unit[3] = {0, 0, 0};    // terms the evaluation reads per matrix, and those with coefficient one
+    std::vector<uint64_t> a_aux_density, b_input_density, b_aux_density;
+    void *d_off = nullptr, *d_idx = nullptr, *d_coef = nullptr, *d_rows = nullptr;
+    uint32_t n_short = 0, n_warp = 0, n_cta = 0;
+    ~bb_r1cs() {
+        for (void* p : {d_off, d_idx, d_coef, d_rows})
+            if (p) ctx->release(p);
+    }
+};
+
+namespace {
+
+int check_witness(const char* fn, const bb_r1cs* R, const void* input, size_t n_inputs, const void* aux, size_t n_aux) {
+    if (n_inputs != R->n_inputs || n_aux != R->n_aux) {
+        set_error("%s: witness has %zu inputs and %zu aux values, the constraint system %zu and %zu", fn, n_inputs, n_aux, R->n_inputs, R->n_aux);
+        return BB_ERR_ARG;
+    }
+    if (!input || (n_aux && !aux)) { set_error("%s: null witness pointer", fn); return BB_ERR_ARG; }
+    return BB_OK;
+}
+
+bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+// queues the evaluation of all 3 N rows on `st`
+int r1cs_eval_queue(bb_ctx* ctx, cudaStream_t st, const bb_r1cs* R, const Fr* d_in, const Fr* d_aux, Fr* oa, Fr* ob, Fr* oc) {
+    EvalArgs A{(const uint32_t*)R->d_off, (const uint32_t*)R->d_idx, (const Fr*)R->d_coef, d_in, d_aux, oa, ob, oc,
+               (uint32_t)R->n_inputs, (uint32_t)R->n};
+    const uint32_t* rows = (const uint32_t*)R->d_rows;
+    if (R->n_short) { k_r1cs_rows_thread<<<cdiv(R->n_short, 128), 128, 0, st>>>(A, rows, R->n_short); ctx->count_launch(); }
+    if (R->n_warp) {
+        k_r1cs_rows_group<32><<<cdiv(R->n_warp, GROUP_THREADS / 32), GROUP_THREADS, 0, st>>>(A, rows + R->n_short, R->n_warp);
+        ctx->count_launch();
+    }
+    if (R->n_cta) {
+        k_r1cs_rows_group<GROUP_THREADS><<<R->n_cta, GROUP_THREADS, 0, st>>>(A, rows + R->n_short + R->n_warp, R->n_cta);
+        ctx->count_launch();
+    }
+    BB_CUDA(cudaGetLastError());
+    return BB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int bb_r1cs_create(bb_ctx* ctx, const bb_r1cs_desc* d, bb_r1cs** out) {
+    if (!ctx || !d || !out) { set_error("bb_r1cs_create: null argument"); return BB_ERR_ARG; }
+    if (d->n_inputs == 0) { set_error("bb_r1cs_create: no inputs (ONE is input 0)"); return BB_ERR_ARG; }
+    const size_t ni = d->n_inputs, nv = d->n_inputs + d->n_aux, rows = d->n_constraints, n = rows + ni;
+    if (nv >= ONE_FLAG || nv < ni) { set_error("bb_r1cs_create: %zu inputs + %zu aux variables: at most 2^31 - 1", ni, d->n_aux); return BB_ERR_ARG; }
+    if (n >= ((size_t)1 << 31) / 3 + 1 || n < rows) { set_error("bb_r1cs_create: %zu constraints: too many", rows); return BB_ERR_ARG; }
+    const bb_r1cs_matrix* mats[3] = {&d->a, &d->b, &d->c};
+    static const char* const name[3] = {"A", "B", "C"};
+    uint64_t total = ni;
+    for (int m = 0; m < 3; m++) {                               // shape first: offsets from 0, non-decreasing
+        const bb_r1cs_matrix& M = *mats[m];
+        if (!M.row_offsets) { set_error("bb_r1cs_create: %s has no row offsets", name[m]); return BB_ERR_ARG; }
+        if (M.row_offsets[0] != 0) { set_error("bb_r1cs_create: %s row_offsets[0] = %llu, not 0", name[m], (unsigned long long)M.row_offsets[0]); return BB_ERR_ARG; }
+        for (size_t k = 0; k < rows; k++)
+            if (M.row_offsets[k + 1] < M.row_offsets[k]) { set_error("bb_r1cs_create: %s row_offsets decrease at row %zu", name[m], k); return BB_ERR_ARG; }
+        const uint64_t terms = M.row_offsets[rows];
+        if (terms && (!M.vars || !M.coeffs)) { set_error("bb_r1cs_create: %s has %llu terms and a null array", name[m], (unsigned long long)terms); return BB_ERR_ARG; }
+        total += terms;
+        if (total >= ((uint64_t)1 << 32)) { set_error("bb_r1cs_create: more than 2^32 - 1 terms"); return BB_ERR_ARG; }
+    }
+    std::unique_ptr<bb_r1cs> R(new bb_r1cs());
+    R->ctx = ctx; R->n_inputs = ni; R->n_aux = d->n_aux; R->n = n;
+    const size_t aux_words = (d->n_aux + 63) / 64, in_words = (ni + 63) / 64;
+    R->a_aux_density.assign(aux_words ? aux_words : 1, 0);
+    R->b_input_density.assign(in_words, 0);
+    R->b_aux_density.assign(aux_words ? aux_words : 1, 0);
+    const Fr one = fr_one();
+    std::vector<uint32_t> off(3 * n + 1), idx, rbins[3];
+    std::vector<Fr> coef;
+    idx.reserve(total);
+    coef.reserve(total);
+    auto bin = [&](uint32_t g, uint64_t len) { rbins[len <= SHORT_MAX ? 0 : len <= WARP_MAX ? 1 : 2].push_back(g); };
+    for (int m = 0; m < 3; m++) {
+        const bb_r1cs_matrix& M = *mats[m];
+        const Fr* cf = (const Fr*)M.coeffs;
+        for (size_t k = 0; k < rows; k++) {
+            const uint32_t g = (uint32_t)(m * n + k);
+            off[g] = (uint32_t)idx.size();
+            for (uint64_t t = M.row_offsets[k]; t < M.row_offsets[k + 1]; t++) {
+                const uint32_t v = M.vars[t];
+                Fr c;
+                std::memcpy(c.l, cf + t, 32);
+                if (v >= nv) { set_error("bb_r1cs_create: %s row %zu term %llu: variable %u of %zu", name[m], k, (unsigned long long)(t - M.row_offsets[k]), v, nv); return BB_ERR_ARG; }
+                if (fr_geq_modulus(c.l)) { set_error("bb_r1cs_create: %s row %zu term %llu: coefficient not below r", name[m], k, (unsigned long long)(t - M.row_offsets[k])); return BB_ERR_ARG; }
+                if (c.is_zero()) continue;                       // eval: a zero coefficient neither adds nor marks (prover.rs:31-44)
+                if (v >= ni) {
+                    if (m == 0) R->a_aux_density[(v - ni) >> 6] |= 1ull << ((v - ni) & 63);
+                    if (m == 1) R->b_aux_density[(v - ni) >> 6] |= 1ull << ((v - ni) & 63);
+                } else if (m == 1) {
+                    R->b_input_density[v >> 6] |= 1ull << (v & 63);
+                }
+                const bool unit = c == one;
+                idx.push_back(v | (unit ? ONE_FLAG : 0u));
+                coef.push_back(c);
+                R->unit[m] += unit;
+            }
+            bin(g, idx.size() - off[g]);
+        }
+        for (size_t i = 0; i < ni; i++) {                        // x_i * 0 = 0 for every input (prover.rs:208-215)
+            const uint32_t g = (uint32_t)(m * n + rows + i);
+            off[g] = (uint32_t)idx.size();
+            if (m == 0) { idx.push_back((uint32_t)i | ONE_FLAG); coef.push_back(one); R->unit[0]++; }
+            bin(g, idx.size() - off[g]);
+        }
+        R->nnz[m] = idx.size() - off[(size_t)m * n];
+    }
+    off[3 * n] = (uint32_t)idx.size();
+    R->n_short = (uint32_t)rbins[0].size(); R->n_warp = (uint32_t)rbins[1].size(); R->n_cta = (uint32_t)rbins[2].size();
+    std::vector<uint32_t> order;
+    order.reserve(3 * n);
+    for (auto& b : rbins) order.insert(order.end(), b.begin(), b.end());
+    BB_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->main_stream;
+    R1csTimer tm(ctx, st);
+    tm.mark("r1cs.begin");
+    BB_TRY(ctx->alloc(off.size() * 4, &R->d_off));
+    BB_TRY(ctx->alloc((idx.size() ? idx.size() : 1) * 4, &R->d_idx));
+    BB_TRY(ctx->alloc((coef.size() ? coef.size() : 1) * 32, &R->d_coef));
+    BB_TRY(ctx->alloc(order.size() * 4, &R->d_rows));
+    BB_CUDA(cudaMemcpyAsync(R->d_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice, st));
+    if (idx.size()) BB_CUDA(cudaMemcpyAsync(R->d_idx, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice, st));
+    if (coef.size()) BB_CUDA(cudaMemcpyAsync(R->d_coef, coef.data(), coef.size() * 32, cudaMemcpyHostToDevice, st));
+    BB_CUDA(cudaMemcpyAsync(R->d_rows, order.data(), order.size() * 4, cudaMemcpyHostToDevice, st));
+    tm.mark("r1cs.upload");
+    BB_CUDA(cudaStreamSynchronize(st));                           // the host vectors go out of scope
+    tm.report(idx.size());
+    *out = R.release();
+    return BB_OK;
+}
+
+void bb_r1cs_destroy(bb_r1cs* r) { delete r; }
+
+int bb_r1cs_info(const bb_r1cs* R, uint64_t* shape, uint64_t* a_aux_density, uint64_t* b_input_density, uint64_t* b_aux_density) {
+    if (!R || !shape) { set_error("bb_r1cs_info: null argument"); return BB_ERR_ARG; }
+    const uint64_t s[BB_R1CS_SHAPE_WORDS] = {R->n, R->n_inputs, R->n_aux, R->nnz[0], R->nnz[1], R->nnz[2], R->unit[0], R->unit[1], R->unit[2]};
+    std::memcpy(shape, s, sizeof s);
+    const size_t aux_words = (R->n_aux + 63) / 64, in_words = (R->n_inputs + 63) / 64;
+    if (a_aux_density) std::memcpy(a_aux_density, R->a_aux_density.data(), aux_words * 8);
+    if (b_input_density) std::memcpy(b_input_density, R->b_input_density.data(), in_words * 8);
+    if (b_aux_density) std::memcpy(b_aux_density, R->b_aux_density.data(), aux_words * 8);
+    return BB_OK;
+}
+
+int bb_r1cs_eval(bb_ctx* ctx, const bb_r1cs* R, const void* input, size_t n_inputs, const void* aux, size_t n_aux, int in_on_device,
+                 void* a, void* b, void* c, int out_on_device) {
+    if (!ctx || !R || !a || !b || !c) { set_error("bb_r1cs_eval: null argument"); return BB_ERR_ARG; }
+    if (R->ctx != ctx) { set_error("bb_r1cs_eval: the constraint system lives on another context"); return BB_ERR_ARG; }
+    BB_TRY(check_witness("bb_r1cs_eval", R, input, n_inputs, aux, n_aux));
+    if ((in_on_device && !(aligned16(input) && aligned16(aux))) || (out_on_device && !(aligned16(a) && aligned16(b) && aligned16(c)))) {
+        set_error("bb_r1cs_eval: device arrays must be 16-byte aligned");
+        return BB_ERR_ARG;
+    }
+    BB_CUDA(cudaSetDevice(ctx->device));
+    NvtxRange nvtx("r1cs_eval");
+    cudaStream_t st = ctx->main_stream;
+    const size_t n = R->n;
+    R1csTimer tm(ctx, st);
+    tm.mark("r1cs.begin");
+    DevBuf d_z, d_out;
+    const Fr *d_in = (const Fr*)input, *d_aux = (const Fr*)aux;
+    if (!in_on_device) {
+        BB_TRY(d_z.alloc(ctx, (n_inputs + n_aux) * 32));
+        BB_CUDA(cudaMemcpyAsync(d_z.p, input, n_inputs * 32, cudaMemcpyHostToDevice, st));
+        if (n_aux) BB_CUDA(cudaMemcpyAsync(d_z.as<Fr>() + n_inputs, aux, n_aux * 32, cudaMemcpyHostToDevice, st));
+        ctx->h2d_bytes += (n_inputs + n_aux) * 32;
+        d_in = d_z.as<Fr>();
+        d_aux = d_z.as<Fr>() + n_inputs;
+    }
+    tm.mark("r1cs.upload");
+    Fr *oa = (Fr*)a, *ob = (Fr*)b, *oc = (Fr*)c;
+    if (!out_on_device) {
+        BB_TRY(d_out.alloc(ctx, 3 * n * 32));
+        oa = d_out.as<Fr>(); ob = oa + n; oc = ob + n;
+    }
+    BB_TRY(r1cs_eval_queue(ctx, st, R, d_in, d_aux, oa, ob, oc));
+    tm.mark("r1cs.eval");
+    if (!out_on_device) {
+        BB_CUDA(cudaMemcpyAsync(a, oa, n * 32, cudaMemcpyDeviceToHost, st));
+        BB_CUDA(cudaMemcpyAsync(b, ob, n * 32, cudaMemcpyDeviceToHost, st));
+        BB_CUDA(cudaMemcpyAsync(c, oc, n * 32, cudaMemcpyDeviceToHost, st));
+        ctx->d2h_bytes += 3 * n * 32;
+    }
+    tm.mark("r1cs.download");
+    BB_CUDA(cudaStreamSynchronize(st));
+    tm.report(R->nnz[0] + R->nnz[1] + R->nnz[2]);
+    return BB_OK;
+}
+
+int bb_groth16_prove_r1cs(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* R, const void* input, size_t n_inputs, const void* aux,
+                          size_t n_aux, int on_device, const uint8_t r[32], const uint8_t s[32], uint8_t proof[192]) {
+    if (!ctx || !crs || !R || !r || !s || !proof) { set_error("bb_groth16_prove_r1cs: null argument"); return BB_ERR_ARG; }
+    if (R->ctx != ctx) { set_error("bb_groth16_prove_r1cs: the constraint system lives on another context"); return BB_ERR_ARG; }
+    BB_TRY(check_witness("bb_groth16_prove_r1cs", R, input, n_inputs, aux, n_aux));
+    if (on_device && !(aligned16(input) && aligned16(aux))) { set_error("bb_groth16_prove_r1cs: device arrays must be 16-byte aligned"); return BB_ERR_ARG; }
+    BB_CUDA(cudaSetDevice(ctx->device));
+    NvtxRange nvtx("prove_r1cs (upload, eval)");
+    cudaStream_t st = ctx->main_stream;
+    const size_t n = R->n;
+    R1csTimer tm(ctx, st);
+    tm.mark("r1cs.begin");
+    DevBuf d_z, d_abc;
+    const Fr *d_in = (const Fr*)input, *d_aux = (const Fr*)aux;
+    if (!on_device) {
+        BB_TRY(d_z.alloc(ctx, (n_inputs + n_aux) * 32));
+        BB_CUDA(cudaMemcpyAsync(d_z.p, input, n_inputs * 32, cudaMemcpyHostToDevice, st));
+        if (n_aux) BB_CUDA(cudaMemcpyAsync(d_z.as<Fr>() + n_inputs, aux, n_aux * 32, cudaMemcpyHostToDevice, st));
+        ctx->h2d_bytes += (n_inputs + n_aux) * 32;
+        d_in = d_z.as<Fr>();
+        d_aux = d_z.as<Fr>() + n_inputs;
+        // the prover copies the assignments on a stream of its own: the upload must be complete before it is called
+        // (the evaluation queued below need not be -- the witness MSMs do not wait for it)
+        BB_CUDA(cudaStreamSynchronize(st));
+    }
+    tm.mark("r1cs.upload");
+    BB_TRY(d_abc.alloc(ctx, 3 * n * 32));
+    Fr* oa = d_abc.as<Fr>();
+    BB_TRY(r1cs_eval_queue(ctx, st, R, d_in, d_aux, oa, oa + n, oa + 2 * n));
+    tm.mark("r1cs.eval");
+    // create_proof from here on (prover.rs:217-360): the H pipeline reads a, b, c on the same stream, after the evaluation
+    bb_witness w{};
+    w.a = oa; w.b = oa + n; w.c = oa + 2 * n; w.n_constraints = n;
+    w.input_assignment = d_in; w.n_inputs = n_inputs;
+    w.aux_assignment = d_aux; w.n_aux = n_aux;
+    w.a_aux_density = R->a_aux_density.data();
+    w.b_input_density = R->b_input_density.data();
+    w.b_aux_density = R->b_aux_density.data();
+    w.on_device = 1;
+    const int rc = bb_groth16_prove(ctx, crs, &w, r, s, proof);
+    if (cudaStreamSynchronize(st) == cudaSuccess) tm.report(R->nnz[0] + R->nnz[1] + R->nnz[2]);
+    return rc;
+}
+
+}  // extern "C"

@@ -184,4 +184,40 @@ int bb_synth_mimc_witness(size_t rounds, uint64_t seed, uint64_t* a, uint64_t* b
     return (n_aux == num_aux && row == 2 * rounds + 2) ? BB_OK : BB_ERR_ARG;
 }
 
+// The matrices of the circuit above, in the order its LinearCombinations push their terms
+// (groth16/tests/common/mod.rs:48-129); the input rows are left to bb_r1cs_create.
+int bb_synth_mimc_r1cs(size_t rounds, uint64_t seed, uint64_t* a_off, uint32_t* a_vars, uint64_t* a_coeffs,
+                       uint64_t* b_off, uint32_t* b_vars, uint64_t* b_coeffs, uint64_t* c_off, uint32_t* c_vars, uint64_t* c_coeffs) {
+    if (!rounds || !a_off || !a_vars || !a_coeffs || !b_off || !b_vars || !b_coeffs || !c_off || !c_vars || !c_coeffs) return BB_ERR_ARG;
+    SplitMix g{seed};
+    std::vector<Fr> constants(rounds);
+    for (auto& k : constants) k = random_fr(g);
+    const Fr one = fr_one(), minus_one = Fr::zero() - fr_one();
+    struct Csr {
+        uint64_t* off; uint32_t* vars; uint64_t* coeffs; size_t row = 0, t = 0;
+        void term(uint32_t v, const Fr& k) { vars[t] = v; put(coeffs, t, k); t++; }
+        void end_row() { off[++row] = t; }
+    } A{a_off, a_vars, a_coeffs}, B{b_off, b_vars, b_coeffs}, C{c_off, c_vars, c_coeffs};
+    a_off[0] = b_off[0] = c_off[0] = 0;
+    const uint32_t ONE = 0, IMAGE = 1, AUX = 2;
+    uint32_t n_aux = 0;
+    uint32_t xl = AUX + n_aux++, xr = AUX + n_aux++;       // preimage xl, xr
+    for (size_t i = 0; i < rounds; i++) {
+        const Fr& ci = constants[i];
+        const uint32_t tmp = AUX + n_aux++;
+        // tmp = (xL + Ci)^2
+        A.term(xl, one); A.term(ONE, ci); A.end_row();
+        B.term(xl, one); B.term(ONE, ci); B.end_row();
+        C.term(tmp, one); C.end_row();
+        const uint32_t nw = i + 1 == rounds ? IMAGE : AUX + n_aux++;
+        // new_xL = xR + tmp*(xL + Ci)
+        A.term(tmp, one); A.end_row();
+        B.term(xl, one); B.term(ONE, ci); B.end_row();
+        C.term(nw, one); C.term(xr, minus_one); C.end_row();
+        xr = xl;
+        xl = nw;
+    }
+    return (n_aux == 2 * rounds + 1 && A.t == 3 * rounds && B.t == 4 * rounds && C.t == 3 * rounds) ? BB_OK : BB_ERR_ARG;
+}
+
 }  // extern "C"

@@ -1,0 +1,190 @@
+"""The constraint system resident on the device (bb_r1cs_*, csrc/r1cs.cu): prove from the witness alone.
+
+ProvingAssignment::enforce (groth16/src/prover.rs:19-55,105-145) evaluates every linear combination of every
+constraint during synthesis.  With the A, B, C matrices in HBM beside the key -- the ones KeypairAssembly records for
+generate_parameters -- a proof needs only input_assignment and aux_assignment; a, b, c and the densities come from the
+device:
+
+    r1cs = R1CS.from_assembly(worker, asm)          # the KeypairAssembly synthesis left, as for generate_parameters
+    proof = create_proof_r1cs(r1cs, params, input_assignment, aux_assignment, r, s)
+
+Matrices are CSR by constraint: (row_offsets uint64 (n+1,), vars uint32 (nnz,), coeffs (nnz, 4) uint64 Montgomery Fr),
+variables numbered inputs first (ONE = 0), then aux.  The input rows of prover.rs:208-215 are appended by the library.
+"""
+import ctypes as C
+
+import numpy as np
+
+from . import EvaluationDomain, _c64, _check, _ptr, _scalar_bytes, load_library
+
+FR_MODULUS = EvaluationDomain.FR_MODULUS
+SHAPE_WORDS = 9
+_MASK64 = (1 << 64) - 1
+
+
+class _Matrix(C.Structure):
+    _fields_ = [("row_offsets", C.c_void_p), ("vars", C.c_void_p), ("coeffs", C.c_void_p)]
+
+
+class _Desc(C.Structure):
+    _fields_ = [("a", _Matrix), ("b", _Matrix), ("c", _Matrix),
+                ("n_constraints", C.c_size_t), ("n_inputs", C.c_size_t), ("n_aux", C.c_size_t)]
+
+
+def _addr(p):
+    return p.value if isinstance(p, C.c_void_p) else int(p)
+
+
+def _unpack(words, n):
+    return np.unpackbits(np.ascontiguousarray(words, np.uint64).view(np.uint8), bitorder="little")[:n].astype(bool)
+
+
+def _mont_limbs(ints):
+    """Python integers mod r -> (n, 4) uint64 Montgomery limbs"""
+    out = np.zeros((len(ints), 4), np.uint64)
+    for i, v in enumerate(ints):
+        m = (v % FR_MODULUS) * (1 << 256) % FR_MODULUS
+        out[i] = [(m >> (64 * j)) & _MASK64 for j in range(4)]
+    return out
+
+
+class R1CS:
+    """bb_r1cs: the A, B, C matrices of one circuit in HBM.  a, b, c: (row_offsets, vars, coeffs) per matrix."""
+
+    def __init__(self, worker, n_inputs, n_aux, a, b, c):
+        mats = []
+        for off, var, cf in (a, b, c):
+            off = np.ascontiguousarray(off, np.uint64)
+            var = np.ascontiguousarray(var, np.uint32)
+            cf = _c64(cf, 4) if len(cf) else np.zeros((0, 4), np.uint64)
+            mats.append((off, var, cf))
+        n = mats[0][0].shape[0] - 1
+        if n < 0 or any(m[0].shape[0] != n + 1 for m in mats):
+            raise ValueError("the three matrices need the same number of rows")
+        d = _Desc()
+        for name, (off, var, cf) in zip("abc", mats):
+            setattr(d, name, _Matrix(off.ctypes.data, var.ctypes.data if var.size else None, cf.ctypes.data if cf.size else None))
+        d.n_constraints, d.n_inputs, d.n_aux = n, n_inputs, n_aux
+        h = C.c_void_p()
+        _check(load_library().bb_r1cs_create(worker._h, C.byref(d), C.byref(h)))
+        self.worker, self._h = worker, h
+        shape = np.zeros(SHAPE_WORDS, np.uint64)
+        _check(load_library().bb_r1cs_info(h, _ptr(shape), None, None, None))
+        self.n_constraints, self.n_inputs, self.n_aux = (int(x) for x in shape[:3])
+        self.nnz = tuple(int(x) for x in shape[3:6])              # terms the evaluation reads, per matrix
+        self.unit = tuple(int(x) for x in shape[6:9])             # of those, coefficient one
+        worker._children.add(self)
+
+    @classmethod
+    def from_assembly(cls, worker, asm):
+        """generator.KeypairAssembly as synthesis leaves it (ONE allocated as input 0, no input rows): its per-variable
+        (coefficient, constraint) lists transposed into rows.  Duplicate and zero-coefficient terms are kept as
+        recorded, so the densities are bellman's."""
+        ni, n = asm.num_inputs, asm.num_constraints
+        mats = []
+        for inputs, aux in ((asm.at_inputs, asm.at_aux), (asm.bt_inputs, asm.bt_aux), (asm.ct_inputs, asm.ct_aux)):
+            rows, vars_, coeffs = [], [], []
+            for base, per_var in ((0, inputs), (ni, aux)):
+                for j, terms in enumerate(per_var):
+                    for coeff, row in terms:
+                        rows.append(row)
+                        vars_.append(base + j)
+                        coeffs.append(coeff)
+            order = np.argsort(np.array(rows, np.int64), kind="stable")
+            off = np.zeros(n + 1, np.uint64)
+            off[1:] = np.cumsum(np.bincount(np.array(rows, np.int64), minlength=n)[:n])
+            cf = _mont_limbs(coeffs)[order] if coeffs else np.zeros((0, 4), np.uint64)
+            mats.append((off, np.array(vars_, np.uint32)[order], cf))
+        return cls(worker, ni, asm.num_aux, *mats)
+
+    @classmethod
+    def synth_mimc(cls, worker, rounds, seed):
+        """bench-only: the MiMC circuit of bb_synth_mimc_witness(rounds, seed) (same constants), from bb_synth_mimc_r1cs"""
+        mats = []
+        for terms in (3 * rounds, 4 * rounds, 3 * rounds):
+            mats.append((np.zeros(2 * rounds + 1, np.uint64), np.zeros(terms, np.uint32), np.zeros((terms, 4), np.uint64)))
+        args = [_ptr(x) for m in mats for x in m]
+        _check(load_library().bb_synth_mimc_r1cs(C.c_size_t(rounds), C.c_uint64(seed), *args))
+        return cls(worker, 2, 2 * rounds + 1, *mats)
+
+    def density_words(self):
+        """(a_aux_density, b_input_density, b_aux_density) as bb_witness's LSB-first uint64 words"""
+        aw, iw = max(1, (self.n_aux + 63) // 64), max(1, (self.n_inputs + 63) // 64)
+        a, bi, b = np.zeros(aw, np.uint64), np.zeros(iw, np.uint64), np.zeros(aw, np.uint64)
+        _check(load_library().bb_r1cs_info(self._h, _ptr(np.zeros(SHAPE_WORDS, np.uint64)), _ptr(a), _ptr(bi), _ptr(b)))
+        return a, bi, b
+
+    def densities(self):
+        """(a_aux_density, b_input_density, b_aux_density) as bool arrays of n_aux, n_inputs, n_aux entries"""
+        a, bi, b = self.density_words()
+        return _unpack(a, self.n_aux), _unpack(bi, self.n_inputs), _unpack(b, self.n_aux)
+
+    def eval(self, input_assignment, aux_assignment, on_device=False, out=None):
+        """a, b, c for the witness (bb_r1cs_eval).  Host arrays of Montgomery Fr, or with on_device=True device addresses
+        (lengths taken from the constraint system).  out: None -> three (n, 4) host arrays returned; or a dict a, b, c
+        of device addresses written in place."""
+        if on_device:
+            src = (C.c_void_p(_addr(input_assignment)), self.n_inputs, C.c_void_p(_addr(aux_assignment)), self.n_aux)
+            keep = ()
+        else:
+            inp, aux = _c64(input_assignment, 4), _c64(aux_assignment, 4)
+            src = (_ptr(inp), inp.shape[0], _ptr(aux), aux.shape[0])
+            keep = (inp, aux)
+        if out is None:
+            res = [np.zeros((self.n_constraints, 4), np.uint64) for _ in range(3)]
+            dst = [_ptr(x) for x in res]
+        else:
+            res = None
+            dst = [C.c_void_p(_addr(out[k])) for k in "abc"]
+        _check(load_library().bb_r1cs_eval(self.worker._h, self._h, src[0], C.c_size_t(src[1]), src[2], C.c_size_t(src[3]),
+                                           C.c_int(1 if on_device else 0), *dst, C.c_int(0 if out is None else 1)))
+        del keep
+        return None if res is None else tuple(res)
+
+    def assignment(self, input_assignment, aux_assignment):
+        """the ProvingAssignment bellman's synthesis would have built, evaluated on the device"""
+        from . import ProvingAssignment
+        a, b, c = self.eval(input_assignment, aux_assignment)
+        asg = ProvingAssignment.__new__(ProvingAssignment)
+        asg.a, asg.b, asg.c = a, b, c
+        asg.input_assignment, asg.aux_assignment = _c64(input_assignment, 4), _c64(aux_assignment, 4)
+        asg.a_aux_density, asg.b_input_density, asg.b_aux_density = self.density_words()
+        return asg
+
+    def free(self):
+        if getattr(self, "_h", None):
+            if getattr(self.worker, "_h", None):
+                load_library().bb_r1cs_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+def create_proof_r1cs(r1cs, params, input_assignment, aux_assignment, r, s, device_ptrs=None):
+    """create_proof from the witness alone (bb_groth16_prove_r1cs): the bytes create_proof gives for the
+    ProvingAssignment synthesis would have built.  device_ptrs: optional dict inputs, aux -> device addresses (the
+    witness resident in HBM; input_assignment / aux_assignment are then ignored)."""
+    if device_ptrs is not None:
+        src = (C.c_void_p(_addr(device_ptrs["inputs"])), r1cs.n_inputs, C.c_void_p(_addr(device_ptrs["aux"])), r1cs.n_aux, 1)
+        keep = ()
+    else:
+        inp, aux = _c64(input_assignment, 4), _c64(aux_assignment, 4)
+        src = (_ptr(inp), inp.shape[0], _ptr(aux), aux.shape[0], 0)
+        keep = (inp, aux)
+    proof = (C.c_uint8 * 192)()
+    _check(load_library().bb_groth16_prove_r1cs(params.worker._h, params._h, r1cs._h, src[0], C.c_size_t(src[1]), src[2],
+                                                C.c_size_t(src[3]), C.c_int(src[4]), _scalar_bytes(r), _scalar_bytes(s), proof))
+    del keep
+    return bytes(proof)
+
+
+def create_random_proof_r1cs(r1cs, params, input_assignment, aux_assignment, rng=None, device_ptrs=None):
+    """create_random_proof (prover.rs:164-179) from the witness alone: r, s <- Fr::random, then create_proof_r1cs"""
+    import secrets
+    draw = rng.randrange if rng is not None else secrets.randbelow
+    return create_proof_r1cs(r1cs, params, input_assignment, aux_assignment, draw(FR_MODULUS), draw(FR_MODULUS), device_ptrs)
+

@@ -85,7 +85,7 @@ void bb_ctx_destroy(bb_ctx* ctx);
  *   msm_precompute_groups  which vectors use the tables: mask of 1 (G1) and 2 (G2), default 3
  *   shard_windows      multi-GPU: window groups per base range (default 4; 1 = base ranges only)
  *   ntt_radix8         1 = register radix-8 NTT windows (default 0: measured slower), ntt_tile_log, ntt_col_bits
- *   profile            1 = CUDA-event timing of the MSM stages, and of the verify.* and decode.* stages (bb_profile_read) */
+ *   profile            1 = CUDA-event timing of the MSM stages, and of the verify.*, decode.* and r1cs.* stages (bb_profile_read) */
 int bb_ctx_set_option(bb_ctx* ctx, const char* key, long value);
 int bb_ctx_synchronize(bb_ctx* ctx);
 /* counters for the harness: number of kernels this context has launched */
@@ -266,6 +266,49 @@ int bb_groth16_finalize_with(const bb_crs* crs, const uint8_t* partials, size_t 
  * b_g1_inputs, b_g1_aux, b_g2_inputs, b_g2_aux, h, l (:339-354). */
 int bb_groth16_prove(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w,
                      const uint8_t r[32], const uint8_t s[32], uint8_t proof[192]);
+
+/* ---- the constraint system on the device: ProvingAssignment::enforce (groth16/src/prover.rs:19-55,105-145) ---------
+ * The A, B, C matrices of a circuit -- what KeypairAssembly records for generate_parameters (generator.rs:43-155) -- kept
+ * in HBM beside the key, so that a proof needs only the witness: a = A z, b = B z, c = C z with
+ * z = input_assignment || aux_assignment are computed on the device and the enforce closures are never called. */
+typedef struct bb_r1cs bb_r1cs;
+/* one matrix in CSR by constraint: row k holds the terms row_offsets[k] .. row_offsets[k+1] - 1 of vars / coeffs.
+ * vars: input i = i, aux j = n_inputs + j.  coeffs: Fr, Montgomery.  Terms are taken as given, unmerged
+ * (LinearCombination + (coeff, var) pushes, src/lib.rs:204-208). */
+typedef struct bb_r1cs_matrix {
+    const uint64_t* row_offsets;   /* n_constraints + 1 entries, row_offsets[0] = 0, non-decreasing */
+    const uint32_t* vars;
+    const void* coeffs;
+} bb_r1cs_matrix;
+typedef struct bb_r1cs_desc {
+    bb_r1cs_matrix a, b, c;
+    size_t n_constraints;          /* the rows the circuit enforced after alloc_input(ONE) (prover.rs:204-206) */
+    size_t n_inputs;               /* including ONE, input 0 */
+    size_t n_aux;
+} bb_r1cs_desc;
+/* Validates the matrices, appends one row per input (A = input_i with coefficient 1, B = C = 0; prover.rs:208-215,
+ * generator.rs:193-202), computes the three densities as eval does (prover.rs:31-44: a term counts only with a non-zero
+ * coefficient; a_aux_density from A, b_input_density and b_aux_density from B; inputs in A and all of C do not count) and
+ * uploads the matrices.  Where bellman would panic on an index, BB_ERR_ARG with a message: n_inputs = 0, row offsets
+ * not starting at 0 or decreasing, a variable >= n_inputs + n_aux, a coefficient >= r, more than 2^32 - 1 terms. */
+int bb_r1cs_create(bb_ctx* ctx, const bb_r1cs_desc* desc, bb_r1cs** out);
+void bb_r1cs_destroy(bb_r1cs* r1cs);
+/* shape[BB_R1CS_SHAPE_WORDS] = n_constraints (incl. the input rows, = bb_witness.n_constraints), n_inputs, n_aux, then
+ * per matrix A, B, C the terms the evaluation reads (non-zero coefficients, incl. the input rows), then per matrix how
+ * many of those have coefficient one.  The densities (any may be NULL) in bb_witness's LSB-first word format. */
+#define BB_R1CS_SHAPE_WORDS 9
+int bb_r1cs_info(const bb_r1cs* r1cs, uint64_t* shape, uint64_t* a_aux_density, uint64_t* b_input_density, uint64_t* b_aux_density);
+/* a, b, c (n_constraints Fr each, Montgomery) = the three products for the witness input (n_inputs Fr) and aux (n_aux
+ * Fr): what ProvingAssignment holds after synthesis.  in_on_device / out_on_device: the witness / the results are device
+ * pointers (16-byte aligned).  Blocking.  BB_ERR_ARG when n_inputs or n_aux differ from the constraint system's. */
+int bb_r1cs_eval(bb_ctx* ctx, const bb_r1cs* r1cs, const void* input, size_t n_inputs, const void* aux, size_t n_aux,
+                 int in_on_device, void* a, void* b, void* c, int out_on_device);
+/* create_proof from the witness alone: the same 192 bytes as bb_groth16_prove for the bb_witness that ProvingAssignment
+ * would have built.  The evaluation runs on the device ahead of the H pipeline; the witness MSMs do not wait for it.  Only
+ * input and aux cross the bus (on_device = 0) or none (on_device != 0).  Argument errors as bb_r1cs_eval, before any
+ * device work; then exactly bb_groth16_prove's errors and their precedence. */
+int bb_groth16_prove_r1cs(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* r1cs, const void* input, size_t n_inputs,
+                          const void* aux, size_t n_aux, int on_device, const uint8_t r[32], const uint8_t s[32], uint8_t proof[192]);
 
 /* ---- verification: groth16/src/verifier.rs and groth16/src/verifier/batch.rs ------------------
  * Points are taken as valid curve and subgroup elements, as the reference's Proof / VerifyingKey types guarantee

@@ -27,6 +27,12 @@ int bb_synth_mimc_shape(size_t rounds, uint64_t shape[7]);
 int bb_synth_mimc_witness(size_t rounds, uint64_t seed, uint64_t* a, uint64_t* b, uint64_t* c,
                           uint64_t* inputs, uint64_t* aux, uint64_t* a_aux_density,
                           uint64_t* b_input_density, uint64_t* b_aux_density);
+/* the constraints bb_synth_mimc_witness's circuit enforces (same constants for the same seed), in bb_r1cs_matrix form
+ * without the input rows (bb_r1cs_create appends them): 2 rounds rows; variables ONE = 0, the image = 1, then aux j = 2 + j.
+ * a_off, b_off, c_off: 2 rounds + 1 offsets each; A holds 3 rounds terms, B 4 rounds, C 3 rounds (vars uint32, coeffs
+ * Montgomery Fr).  Host code. */
+int bb_synth_mimc_r1cs(size_t rounds, uint64_t seed, uint64_t* a_off, uint32_t* a_vars, uint64_t* a_coeffs,
+                       uint64_t* b_off, uint32_t* b_vars, uint64_t* b_coeffs, uint64_t* c_off, uint32_t* c_vars, uint64_t* c_coeffs);
 
 /* ---- diagnostics (used by the parity tests; not part of the bellman-facing surface) ------ */
 /* element-wise on the device: field 0 = Fr, 1 = Fp (Montgomery); op 0 mul, 1 add, 2 sub, 3 sqr;

@@ -11,6 +11,7 @@ use std::os::raw::{c_char, c_int, c_long, c_void};
 #[repr(C)] pub struct bb_crs { _private: [u8; 0] }
 #[repr(C)] pub struct bb_prove { _private: [u8; 0] }
 #[repr(C)] pub struct bb_vk { _private: [u8; 0] }
+#[repr(C)] pub struct bb_r1cs { _private: [u8; 0] }
 
 // bb_status
 pub const BB_OK: c_int = 0;
@@ -73,6 +74,19 @@ pub struct bb_proof_batch {
     pub inputs: *const c_void, pub n_inputs: usize,
     pub on_device: c_int,
 }
+
+#[repr(C)]
+pub struct bb_r1cs_matrix {
+    pub row_offsets: *const u64, pub vars: *const u32, pub coeffs: *const c_void,
+}
+
+#[repr(C)]
+pub struct bb_r1cs_desc {
+    pub a: bb_r1cs_matrix, pub b: bb_r1cs_matrix, pub c: bb_r1cs_matrix,
+    pub n_constraints: usize, pub n_inputs: usize, pub n_aux: usize,
+}
+
+pub const BB_R1CS_SHAPE_WORDS: usize = 9;
 
 // Proof::read status byte: (which << 4) | why, which 1 = A, 2 = B, 3 = C
 pub const BB_PROOF_BYTES: usize = 192;
@@ -153,6 +167,14 @@ extern "C" {
                                     static_in: *const u8, proof: *mut u8) -> c_int;
     pub fn bb_groth16_prove(ctx: *mut bb_ctx, crs: *const bb_crs, w: *const bb_witness, r: *const u8, s: *const u8,
                             proof: *mut u8) -> c_int;
+    pub fn bb_r1cs_create(ctx: *mut bb_ctx, desc: *const bb_r1cs_desc, out: *mut *mut bb_r1cs) -> c_int;
+    pub fn bb_r1cs_destroy(r1cs: *mut bb_r1cs);
+    pub fn bb_r1cs_info(r1cs: *const bb_r1cs, shape: *mut u64, a_aux_density: *mut u64, b_input_density: *mut u64,
+                        b_aux_density: *mut u64) -> c_int;
+    pub fn bb_r1cs_eval(ctx: *mut bb_ctx, r1cs: *const bb_r1cs, input: *const c_void, n_inputs: usize, aux: *const c_void,
+                        n_aux: usize, in_on_device: c_int, a: *mut c_void, b: *mut c_void, c: *mut c_void, out_on_device: c_int) -> c_int;
+    pub fn bb_groth16_prove_r1cs(ctx: *mut bb_ctx, crs: *const bb_crs, r1cs: *const bb_r1cs, input: *const c_void, n_inputs: usize,
+                                 aux: *const c_void, n_aux: usize, on_device: c_int, r: *const u8, s: *const u8, proof: *mut u8) -> c_int;
 
     pub fn bb_vk_prepare(ctx: *mut bb_ctx, desc: *const bb_vk_desc, out: *mut *mut bb_vk) -> c_int;
     pub fn bb_vk_destroy(vk: *mut bb_vk);

@@ -9,7 +9,7 @@ use std::ptr;
 use std::sync::Arc;
 
 use bellman::groth16::{Parameters, Proof, VerifyingKey};
-use bellman::{SynthesisError, VerificationError};
+use bellman::{Circuit, ConstraintSystem, Index, LinearCombination, SynthesisError, VerificationError, Variable};
 use bellman_b200_sys::*;
 use bls12_381::{Bls12, G1Affine, G1Projective, G2Affine, G2Projective, Scalar};
 use ff::{Field, PrimeField};
@@ -228,6 +228,115 @@ impl GpuParameters {
         status(unsafe { bb_groth16_autotune(self.ctx, self.handle, &wit, reps, &mut chosen, ms.as_mut_ptr()) })?;
         Ok((chosen as usize, ms))
     }
+}
+
+/// The constraint system on the device (bb_r1cs_*): the A, B, C matrices of a circuit kept in HBM beside the key, so that
+/// a proof needs only the witness -- `ProvingAssignment::enforce` (groth16/src/prover.rs:105-145) is never run.
+pub struct GpuR1cs { pub(crate) ctx: *mut bb_ctx, pub(crate) handle: *mut bb_r1cs, n_inputs: usize, n_aux: usize }
+unsafe impl Send for GpuR1cs {}
+unsafe impl Sync for GpuR1cs {}
+
+/// Records what `KeypairAssembly` records (generator.rs:43-155), by constraint: each row's terms as the circuit pushed
+/// them, unmerged.  The witness closures are not called.
+
+struct R1csRecorder { n_inputs: usize, n_aux: usize, rows: usize, m: [(Vec<u64>, Vec<Index>, Vec<Scalar>); 3] }
+impl ConstraintSystem<Scalar> for R1csRecorder {
+    type Root = Self;
+    fn alloc<F, A, AR>(&mut self, _: A, _: F) -> Result<Variable, SynthesisError>
+    where F: FnOnce() -> Result<Scalar, SynthesisError>, A: FnOnce() -> AR, AR: Into<String> {
+        self.n_aux += 1;
+        Ok(Variable::new_unchecked(Index::Aux(self.n_aux - 1)))
+    }
+    fn alloc_input<F, A, AR>(&mut self, _: A, _: F) -> Result<Variable, SynthesisError>
+    where F: FnOnce() -> Result<Scalar, SynthesisError>, A: FnOnce() -> AR, AR: Into<String> {
+        self.n_inputs += 1;
+        Ok(Variable::new_unchecked(Index::Input(self.n_inputs - 1)))
+    }
+    fn enforce<A, AR, LA, LB, LC>(&mut self, _: A, a: LA, b: LB, c: LC)
+    where A: FnOnce() -> AR, AR: Into<String>, LA: FnOnce(LinearCombination<Scalar>) -> LinearCombination<Scalar>,
+          LB: FnOnce(LinearCombination<Scalar>) -> LinearCombination<Scalar>, LC: FnOnce(LinearCombination<Scalar>) -> LinearCombination<Scalar> {
+        let lcs = [a(LinearCombination::zero()), b(LinearCombination::zero()), c(LinearCombination::zero())];
+        for (lc, m) in lcs.iter().zip(self.m.iter_mut()) {
+            for (v, coeff) in lc.as_ref() {
+                m.1.push(v.get_unchecked());
+                m.2.push(*coeff);
+            }
+            m.0.push(m.1.len() as u64);
+        }
+        self.rows += 1;
+    }
+    fn push_namespace<NR, N>(&mut self, _: N) where NR: Into<String>, N: FnOnce() -> NR {}
+    fn pop_namespace(&mut self) {}
+    fn get_root(&mut self) -> &mut Self::Root { self }
+}
+
+/// Runs the `alloc` / `alloc_input` closures of a circuit and never the `enforce` closures: the witness alone.
+#[derive(Default)]
+pub struct WitnessCS { pub input_assignment: Vec<Scalar>, pub aux_assignment: Vec<Scalar> }
+
+impl ConstraintSystem<Scalar> for WitnessCS {
+    type Root = Self;
+    fn alloc<F, A, AR>(&mut self, _: A, f: F) -> Result<Variable, SynthesisError>
+    where F: FnOnce() -> Result<Scalar, SynthesisError>, A: FnOnce() -> AR, AR: Into<String> {
+        self.aux_assignment.push(f()?);
+        Ok(Variable::new_unchecked(Index::Aux(self.aux_assignment.len() - 1)))
+    }
+    fn alloc_input<F, A, AR>(&mut self, _: A, f: F) -> Result<Variable, SynthesisError>
+    where F: FnOnce() -> Result<Scalar, SynthesisError>, A: FnOnce() -> AR, AR: Into<String> {
+        self.input_assignment.push(f()?);
+        Ok(Variable::new_unchecked(Index::Input(self.input_assignment.len() - 1)))
+    }
+    fn enforce<A, AR, LA, LB, LC>(&mut self, _: A, _: LA, _: LB, _: LC)
+    where A: FnOnce() -> AR, AR: Into<String>, LA: FnOnce(LinearCombination<Scalar>) -> LinearCombination<Scalar>,
+          LB: FnOnce(LinearCombination<Scalar>) -> LinearCombination<Scalar>, LC: FnOnce(LinearCombination<Scalar>) -> LinearCombination<Scalar> {}
+    fn push_namespace<NR, N>(&mut self, _: N) where NR: Into<String>, N: FnOnce() -> NR {}
+    fn pop_namespace(&mut self) {}
+    fn get_root(&mut self) -> &mut Self::Root { self }
+}
+
+impl GpuR1cs {
+    /// Synthesises `circuit` once for its shape (after `alloc_input(ONE)`, as prover.rs:204-206 and generator.rs:188 do)
+    /// and uploads the matrices.  The input rows are appended by the library.  The shape must not depend on witness
+    /// values -- which R1CS already requires, since the key is made from one synthesis too.
+    pub fn synthesize<C: Circuit<Scalar>>(worker: &GpuWorker, circuit: C) -> Result<Self, SynthesisError> {
+        let mut cs = R1csRecorder { n_inputs: 0, n_aux: 0, rows: 0, m: Default::default() };
+        for m in cs.m.iter_mut() { m.0.push(0); }
+        cs.alloc_input(|| "", || Ok(Scalar::one()))?;
+        circuit.synthesize(&mut cs)?;
+        let (ni, na) = (cs.n_inputs, cs.n_aux);
+        // variables as the ABI numbers them: inputs first, then aux (an index too large for u32 is left to bb_r1cs_create)
+        let vars: Vec<Vec<u32>> = cs.m.iter()
+            .map(|m| m.1.iter().map(|v| match v { Index::Input(i) => *i as u32, Index::Aux(i) => (ni + i).min(u32::MAX as usize) as u32 }).collect())
+            .collect();
+        let mat = |k: usize| bb_r1cs_matrix {
+            row_offsets: cs.m[k].0.as_ptr(), vars: vars[k].as_ptr(), coeffs: cs.m[k].2.as_ptr() as *const c_void,   // Scalar = Montgomery limbs
+        };
+        let desc = bb_r1cs_desc { a: mat(0), b: mat(1), c: mat(2), n_constraints: cs.rows, n_inputs: ni, n_aux: na };
+        let mut handle = ptr::null_mut();
+        status(unsafe { bb_r1cs_create(worker.ctx, &desc, &mut handle) })?;
+        Ok(GpuR1cs { ctx: worker.ctx, handle, n_inputs: ni, n_aux: na })
+    }
+}
+impl Drop for GpuR1cs {
+    fn drop(&mut self) { unsafe { bb_r1cs_destroy(self.handle) } }
+}
+
+/// `groth16::create_proof` (groth16/src/prover.rs:182-360) with the constraint system on the device: synthesis runs only
+/// the witness closures (`WitnessCS`); a, b, c and the densities are computed from `r1cs` on the device.  The same bytes
+/// as `create_proof_b200` on the `ProvingAssignment` bellman's synthesis would build.
+pub fn create_proof_r1cs_b200<C: Circuit<Scalar>>(circuit: C, r1cs: &GpuR1cs, crs: &GpuParameters, r: Scalar, s: Scalar)
+    -> Result<Proof<Bls12>, SynthesisError> {
+    let mut cs = WitnessCS::default();
+    cs.alloc_input(|| "", || Ok(Scalar::one()))?;
+    circuit.synthesize(&mut cs)?;
+    assert_eq!((cs.input_assignment.len(), cs.aux_assignment.len()), (r1cs.n_inputs, r1cs.n_aux), "the circuit's shape changed");
+    let mut bytes = [0u8; 192];
+    status(unsafe {
+        bb_groth16_prove_r1cs(crs.ctx, crs.handle, r1cs.handle, cs.input_assignment.as_ptr() as _, cs.input_assignment.len(),
+                              cs.aux_assignment.as_ptr() as _, cs.aux_assignment.len(), 0, r.to_repr().as_ptr(), s.to_repr().as_ptr(),
+                              bytes.as_mut_ptr())
+    })?;
+    Proof::read(&bytes[..]).map_err(Into::into)
 }
 
 /// Drop-in for the body of `groth16::create_proof` after synthesis (groth16/src/prover.rs:217-360).
