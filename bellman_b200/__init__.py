@@ -85,6 +85,12 @@ def _ptr(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+def _addr(p):
+    """device address as an int (None for a null one), from an int or a ctypes void pointer (Worker.device_alloc returns
+    the latter)"""
+    return p.value if isinstance(p, C.c_void_p) else None if p is None else int(p)
+
+
 def _c64(a, width):
     a = np.ascontiguousarray(a, dtype=np.uint64)
     return a.reshape(-1, width)
@@ -110,7 +116,7 @@ class Worker:
         _check(lib.bb_ctx_create(C.c_int(device), C.byref(h)))
         self._h = h
         self.device = device
-        self._children = weakref.WeakSet()      # Bases / Parameters living on this context
+        self._children = weakref.WeakSet()      # the _DeviceObjects living on this context
 
     def close(self):
         if getattr(self, "_h", None):
@@ -165,8 +171,33 @@ class Worker:
         _check(load_library().bb_device_download(self._h, _ptr(host_array), d_ptr, C.c_size_t(host_array.nbytes)))
 
 
-class Bases:
+class _DeviceObject:
+    """An object living on a Worker's context: freed by free(), when collected, or with the Worker (close() frees its
+    children before the context).  A subclass names its destroy call in _destroy and calls _own once it holds a handle."""
+
+    _destroy = None
+
+    def _own(self, worker, h):
+        self.worker, self._h = worker, h
+        worker._children.add(self)
+
+    def free(self):
+        if getattr(self, "_h", None):
+            if getattr(self.worker, "_h", None):     # a context that is already gone took the device memory with it
+                getattr(load_library(), self._destroy)(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+class Bases(_DeviceObject):
     """Arc<Vec<G::Affine>> resident in HBM (a SourceBuilder's backing store, multiexp.rs:45-51)."""
+
+    _destroy = "bb_bases_free"
 
     def __init__(self, worker, group, points, global_offset=0, global_len=None):
         width = 12 if group == G1 else 24
@@ -177,8 +208,7 @@ class Bases:
         h = C.c_void_p()
         _check(load_library().bb_bases_upload(worker._h, C.c_int(group), _ptr(pts), C.c_size_t(pts.shape[0]),
                                               C.c_size_t(global_offset), C.c_size_t(global_len), C.byref(h)))
-        self._h = h
-        worker._children.add(self)
+        self._own(worker, h)
 
     @classmethod
     def synthetic(cls, worker, group, seed, n, global_offset=0, global_len=None):
@@ -188,8 +218,7 @@ class Bases:
         h = C.c_void_p()
         _check(load_library().bb_synth_bases(worker._h, C.c_int(group), C.c_uint64(seed), C.c_size_t(n), C.c_size_t(global_offset),
                                              C.c_size_t(n if global_len is None else global_len), C.byref(h)))
-        self._h = h
-        worker._children.add(self)
+        self._own(worker, h)
         return self
 
     def precompute(self):
@@ -201,18 +230,6 @@ class Bases:
         """bb_bases_drop_table: frees the window multiples again (no MSM over these bases may be in flight)"""
         _check(load_library().bb_bases_drop_table(self._h))
         return self
-
-    def free(self):
-        if getattr(self, "_h", None):
-            if getattr(self.worker, "_h", None):     # a context that is already gone took the device memory with it
-                load_library().bb_bases_free(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.free()
-        except Exception:
-            pass
 
 
 class _FullDensity:
@@ -411,9 +428,11 @@ class _Witness(C.Structure):
                 ("on_device", C.c_int)]
 
 
-class Parameters:
+class Parameters(_DeviceObject):
     """groth16::Parameters made device-resident (groth16/src/lib.rs:222-244).  `p` maps
     vk_g1 (alpha,beta,delta), vk_g2 (beta,gamma,delta), h, l, a, b_g1, b_g2 to uint64 arrays."""
+
+    _destroy = "bb_crs_destroy"
 
     def __init__(self, worker, p, shard_index=0, shard_count=1):
         self.worker = worker
@@ -432,9 +451,8 @@ class Parameters:
         d.shard_index, d.shard_count = shard_index, shard_count
         h = C.c_void_p()
         _check(load_library().bb_crs_create(worker._h, C.byref(d), C.byref(h)))
-        self._h = h
+        self._own(worker, h)
         self._keep = None                    # the vectors are resident in HBM now
-        worker._children.add(self)
 
     @classmethod
     def synthetic(cls, worker, seed, shape, shard_index=0, shard_count=1):
@@ -447,8 +465,7 @@ class Parameters:
                                            C.c_size_t(shape["num_inputs"] + shape["a_aux_total"]),
                                            C.c_size_t(shape["b_in_total"] + shape["b_aux_total"]),
                                            C.c_uint32(shard_index), C.c_uint32(shard_count), C.byref(h)))
-        self._h = h
-        worker._children.add(self)
+        self._own(worker, h)
         return self
 
     def precompute(self):
@@ -477,18 +494,6 @@ class Parameters:
         _check(lib.bb_groth16_autotune(self.worker._h, self._h, C.byref(w), C.c_int(reps), C.byref(chosen), ms))
         return {"chosen": chosen.value, "name": tuning_names()[chosen.value], "ms": [round(float(x), 3) for x in ms]}
 
-    def free(self):
-        if getattr(self, "_h", None):
-            if getattr(self.worker, "_h", None):     # (the garbage collector may finalise a Worker before its children)
-                load_library().bb_crs_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.free()
-        except Exception:
-            pass
-
 
 def tuning_names():
     """the MSM forms bb_groth16_autotune chooses from (index 0 = default)"""
@@ -510,24 +515,18 @@ class ProvingAssignment:
 
     def _struct(self, device_ptrs=None):
         """device_ptrs: optional dict a,b,c,inputs,aux -> device addresses (inputs resident in HBM)"""
+        p = device_ptrs if device_ptrs is not None else {
+            "a": self.a.ctypes.data, "b": self.b.ctypes.data, "c": self.c.ctypes.data,
+            "inputs": self.input_assignment.ctypes.data, "aux": self.aux_assignment.ctypes.data}
         w = _Witness()
-        if device_ptrs is not None:
-            w.a, w.b, w.c = device_ptrs["a"], device_ptrs["b"], device_ptrs["c"]
-            w.n_constraints = self.a.shape[0]
-            w.input_assignment, w.n_inputs = device_ptrs["inputs"], self.input_assignment.shape[0]
-            w.aux_assignment, w.n_aux = device_ptrs["aux"], self.aux_assignment.shape[0]
-            w.a_aux_density = self.a_aux_density.ctypes.data
-            w.b_input_density = self.b_input_density.ctypes.data
-            w.b_aux_density = self.b_aux_density.ctypes.data
-            w.on_device = 1
-            return w
-        w.a, w.b, w.c = self.a.ctypes.data, self.b.ctypes.data, self.c.ctypes.data
+        w.a, w.b, w.c = p["a"], p["b"], p["c"]
         w.n_constraints = self.a.shape[0]
-        w.input_assignment, w.n_inputs = self.input_assignment.ctypes.data, self.input_assignment.shape[0]
-        w.aux_assignment, w.n_aux = self.aux_assignment.ctypes.data, self.aux_assignment.shape[0]
+        w.input_assignment, w.n_inputs = p["inputs"], self.input_assignment.shape[0]
+        w.aux_assignment, w.n_aux = p["aux"], self.aux_assignment.shape[0]
         w.a_aux_density = self.a_aux_density.ctypes.data
         w.b_input_density = self.b_input_density.ctypes.data
         w.b_aux_density = self.b_aux_density.ctypes.data
+        w.on_device = 0 if device_ptrs is None else 1
         return w
 
 
@@ -550,11 +549,6 @@ def prove_begin(assignment, params, device_ptrs=None):
     h = C.c_void_p()
     _check(load_library().bb_groth16_prove_begin(params.worker._h, params._h, C.byref(w), C.byref(h)))
     return h
-
-
-def _addr(p):
-    """device address as an int, from an int or a ctypes void pointer (Worker.device_alloc returns the latter)"""
-    return p.value if isinstance(p, C.c_void_p) else int(p)
 
 
 def prove_end(state, evals=None):

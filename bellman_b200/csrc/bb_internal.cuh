@@ -139,6 +139,41 @@ struct DevBuf {
     template <class T> T* as() const { return (T*)p; }
 };
 
+// The caller's array on the device: `p` itself when it is in device memory, else a copy queued on `st` into `buf`
+// (counted in h2d_bytes)
+template <class T>
+int device_input(bb_ctx* ctx, cudaStream_t st, const void* p, size_t bytes, bool on_device, DevBuf& buf, const T** out) {
+    if (on_device) { *out = (const T*)p; return BB_OK; }
+    BB_TRY(buf.alloc(ctx, bytes));
+    if (bytes) BB_CUDA(cudaMemcpyAsync(buf.p, p, bytes, cudaMemcpyHostToDevice, st));
+    ctx->h2d_bytes += bytes;
+    *out = buf.as<T>();
+    return BB_OK;
+}
+
+// CUDA-event brackets of a call's stages (profile mode only)
+struct StageTimer {
+    bb_ctx* ctx;
+    cudaStream_t st;
+    std::vector<std::pair<const char*, cudaEvent_t>> marks;
+    StageTimer(bb_ctx* c, cudaStream_t s) : ctx(c), st(s) {}
+    ~StageTimer() { for (auto& m : marks) cudaEventDestroy(m.second); }
+    void mark(const char* stage_ending_here) {
+        if (!ctx->opt_profile) return;
+        cudaEvent_t e;
+        if (cudaEventCreate(&e) != cudaSuccess) return;
+        cudaEventRecord(e, st);
+        marks.emplace_back(stage_ending_here, e);
+    }
+    // after the stream has drained: stage k = the interval between marks k-1 and k
+    void report(uint64_t units) {
+        for (size_t k = 1; k < marks.size(); k++) {
+            float ms = 0;
+            if (cudaEventElapsedTime(&ms, marks[k - 1].second, marks[k].second) == cudaSuccess) ctx->prof_add(marks[k].first, ms, 1, units);
+        }
+    }
+};
+
 inline unsigned cdiv(size_t a, size_t b) { return (unsigned)((a + b - 1) / b); }
 
 // ---- ntt.cu ----

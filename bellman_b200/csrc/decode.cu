@@ -236,28 +236,6 @@ __global__ void __launch_bounds__(128) k_encode_proofs(const G1Affine* __restric
     g1_encode(c[i], o + 144);
 }
 
-// CUDA-event brackets of the stages (profile mode only), as in verify.cu
-struct DecodeTimer {
-    bb_ctx* ctx;
-    cudaStream_t st;
-    std::vector<std::pair<const char*, cudaEvent_t>> marks;
-    DecodeTimer(bb_ctx* c, cudaStream_t s) : ctx(c), st(s) {}
-    ~DecodeTimer() { for (auto& m : marks) cudaEventDestroy(m.second); }
-    void mark(const char* stage_ending_here) {
-        if (!ctx->opt_profile) return;
-        cudaEvent_t e;
-        if (cudaEventCreate(&e) != cudaSuccess) return;
-        cudaEventRecord(e, st);
-        marks.emplace_back(stage_ending_here, e);
-    }
-    void report(uint64_t units) {
-        for (size_t k = 1; k < marks.size(); k++) {
-            float ms = 0;
-            if (cudaEventElapsedTime(&ms, marks[k - 1].second, marks[k].second) == cudaSuccess) ctx->prof_add(marks[k].first, ms, 1, units);
-        }
-    }
-};
-
 constexpr size_t MAX_PROOFS = (size_t)1 << 31;
 
 }  // namespace
@@ -275,7 +253,7 @@ int bb_proofs_read(bb_ctx* ctx, const bb_proof_bytes* in, void* a, void* b, void
     BB_CUDA(cudaSetDevice(ctx->device));
     NvtxRange nvtx("proofs_read");
     cudaStream_t st = ctx->main_stream;
-    DecodeTimer tm(ctx, st);
+    StageTimer tm(ctx, st);
     tm.mark("decode.begin");
     const uint8_t* src = (const uint8_t*)in->bytes;
     size_t src_stride = stride;

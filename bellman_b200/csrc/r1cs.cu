@@ -88,28 +88,6 @@ bool fr_geq_modulus(const uint32_t* v) {
     return true;
 }
 
-// CUDA-event brackets of the stages (profile mode only), as in decode.cu
-struct R1csTimer {
-    bb_ctx* ctx;
-    cudaStream_t st;
-    std::vector<std::pair<const char*, cudaEvent_t>> marks;
-    R1csTimer(bb_ctx* c, cudaStream_t s) : ctx(c), st(s) {}
-    ~R1csTimer() { for (auto& m : marks) cudaEventDestroy(m.second); }
-    void mark(const char* stage_ending_here) {
-        if (!ctx->opt_profile) return;
-        cudaEvent_t e;
-        if (cudaEventCreate(&e) != cudaSuccess) return;
-        cudaEventRecord(e, st);
-        marks.emplace_back(stage_ending_here, e);
-    }
-    void report(uint64_t units) {
-        for (size_t k = 1; k < marks.size(); k++) {
-            float ms = 0;
-            if (cudaEventElapsedTime(&ms, marks[k - 1].second, marks[k].second) == cudaSuccess) ctx->prof_add(marks[k].first, ms, 1, units);
-        }
-    }
-};
-
 }  // namespace
 
 struct bb_r1cs {
@@ -127,16 +105,30 @@ struct bb_r1cs {
 
 namespace {
 
-int check_witness(const char* fn, const bb_r1cs* R, const void* input, size_t n_inputs, const void* aux, size_t n_aux) {
+bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+// The witness checks of eval and prove.  outputs_aligned: the caller's device outputs, if any, are 16-byte aligned.
+int check_witness(const char* fn, const bb_ctx* ctx, const bb_r1cs* R, const void* input, size_t n_inputs, const void* aux, size_t n_aux,
+                  int on_device, bool outputs_aligned) {
+    if (R->ctx != ctx) { set_error("%s: the constraint system lives on another context", fn); return BB_ERR_ARG; }
     if (n_inputs != R->n_inputs || n_aux != R->n_aux) {
         set_error("%s: witness has %zu inputs and %zu aux values, the constraint system %zu and %zu", fn, n_inputs, n_aux, R->n_inputs, R->n_aux);
         return BB_ERR_ARG;
     }
     if (!input || (n_aux && !aux)) { set_error("%s: null witness pointer", fn); return BB_ERR_ARG; }
+    if ((on_device && !(aligned16(input) && aligned16(aux))) || !outputs_aligned) {
+        set_error("%s: device arrays must be 16-byte aligned", fn);
+        return BB_ERR_ARG;
+    }
     return BB_OK;
 }
 
-bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+// z = input || aux on the device: the caller's arrays, or their upload on `st`
+int stage_witness(bb_ctx* ctx, cudaStream_t st, const void* input, size_t n_inputs, const void* aux, size_t n_aux, int on_device,
+                  DevBuf (&up)[2], const Fr** d_in, const Fr** d_aux) {
+    BB_TRY(device_input(ctx, st, input, n_inputs * 32, on_device, up[0], d_in));
+    return device_input(ctx, st, aux, n_aux * 32, on_device, up[1], d_aux);
+}
 
 // queues the evaluation of all 3 N rows on `st`
 int r1cs_eval_queue(bb_ctx* ctx, cudaStream_t st, const bb_r1cs* R, const Fr* d_in, const Fr* d_aux, Fr* oa, Fr* ob, Fr* oc) {
@@ -233,7 +225,7 @@ int bb_r1cs_create(bb_ctx* ctx, const bb_r1cs_desc* d, bb_r1cs** out) {
     for (auto& b : rbins) order.insert(order.end(), b.begin(), b.end());
     BB_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->main_stream;
-    R1csTimer tm(ctx, st);
+    StageTimer tm(ctx, st);
     tm.mark("r1cs.begin");
     BB_TRY(ctx->alloc(off.size() * 4, &R->d_off));
     BB_TRY(ctx->alloc((idx.size() ? idx.size() : 1) * 4, &R->d_idx));
@@ -266,28 +258,17 @@ int bb_r1cs_info(const bb_r1cs* R, uint64_t* shape, uint64_t* a_aux_density, uin
 int bb_r1cs_eval(bb_ctx* ctx, const bb_r1cs* R, const void* input, size_t n_inputs, const void* aux, size_t n_aux, int in_on_device,
                  void* a, void* b, void* c, int out_on_device) {
     if (!ctx || !R || !a || !b || !c) { set_error("bb_r1cs_eval: null argument"); return BB_ERR_ARG; }
-    if (R->ctx != ctx) { set_error("bb_r1cs_eval: the constraint system lives on another context"); return BB_ERR_ARG; }
-    BB_TRY(check_witness("bb_r1cs_eval", R, input, n_inputs, aux, n_aux));
-    if ((in_on_device && !(aligned16(input) && aligned16(aux))) || (out_on_device && !(aligned16(a) && aligned16(b) && aligned16(c)))) {
-        set_error("bb_r1cs_eval: device arrays must be 16-byte aligned");
-        return BB_ERR_ARG;
-    }
+    BB_TRY(check_witness("bb_r1cs_eval", ctx, R, input, n_inputs, aux, n_aux, in_on_device,
+                         !out_on_device || (aligned16(a) && aligned16(b) && aligned16(c))));
     BB_CUDA(cudaSetDevice(ctx->device));
     NvtxRange nvtx("r1cs_eval");
     cudaStream_t st = ctx->main_stream;
     const size_t n = R->n;
-    R1csTimer tm(ctx, st);
+    StageTimer tm(ctx, st);
     tm.mark("r1cs.begin");
-    DevBuf d_z, d_out;
-    const Fr *d_in = (const Fr*)input, *d_aux = (const Fr*)aux;
-    if (!in_on_device) {
-        BB_TRY(d_z.alloc(ctx, (n_inputs + n_aux) * 32));
-        BB_CUDA(cudaMemcpyAsync(d_z.p, input, n_inputs * 32, cudaMemcpyHostToDevice, st));
-        if (n_aux) BB_CUDA(cudaMemcpyAsync(d_z.as<Fr>() + n_inputs, aux, n_aux * 32, cudaMemcpyHostToDevice, st));
-        ctx->h2d_bytes += (n_inputs + n_aux) * 32;
-        d_in = d_z.as<Fr>();
-        d_aux = d_z.as<Fr>() + n_inputs;
-    }
+    DevBuf up[2], d_out;
+    const Fr *d_in, *d_aux;
+    BB_TRY(stage_witness(ctx, st, input, n_inputs, aux, n_aux, in_on_device, up, &d_in, &d_aux));
     tm.mark("r1cs.upload");
     Fr *oa = (Fr*)a, *ob = (Fr*)b, *oc = (Fr*)c;
     if (!out_on_device) {
@@ -311,28 +292,19 @@ int bb_r1cs_eval(bb_ctx* ctx, const bb_r1cs* R, const void* input, size_t n_inpu
 int bb_groth16_prove_r1cs(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* R, const void* input, size_t n_inputs, const void* aux,
                           size_t n_aux, int on_device, const uint8_t r[32], const uint8_t s[32], uint8_t proof[192]) {
     if (!ctx || !crs || !R || !r || !s || !proof) { set_error("bb_groth16_prove_r1cs: null argument"); return BB_ERR_ARG; }
-    if (R->ctx != ctx) { set_error("bb_groth16_prove_r1cs: the constraint system lives on another context"); return BB_ERR_ARG; }
-    BB_TRY(check_witness("bb_groth16_prove_r1cs", R, input, n_inputs, aux, n_aux));
-    if (on_device && !(aligned16(input) && aligned16(aux))) { set_error("bb_groth16_prove_r1cs: device arrays must be 16-byte aligned"); return BB_ERR_ARG; }
+    BB_TRY(check_witness("bb_groth16_prove_r1cs", ctx, R, input, n_inputs, aux, n_aux, on_device, true));
     BB_CUDA(cudaSetDevice(ctx->device));
     NvtxRange nvtx("prove_r1cs (upload, eval)");
     cudaStream_t st = ctx->main_stream;
     const size_t n = R->n;
-    R1csTimer tm(ctx, st);
+    StageTimer tm(ctx, st);
     tm.mark("r1cs.begin");
-    DevBuf d_z, d_abc;
-    const Fr *d_in = (const Fr*)input, *d_aux = (const Fr*)aux;
-    if (!on_device) {
-        BB_TRY(d_z.alloc(ctx, (n_inputs + n_aux) * 32));
-        BB_CUDA(cudaMemcpyAsync(d_z.p, input, n_inputs * 32, cudaMemcpyHostToDevice, st));
-        if (n_aux) BB_CUDA(cudaMemcpyAsync(d_z.as<Fr>() + n_inputs, aux, n_aux * 32, cudaMemcpyHostToDevice, st));
-        ctx->h2d_bytes += (n_inputs + n_aux) * 32;
-        d_in = d_z.as<Fr>();
-        d_aux = d_z.as<Fr>() + n_inputs;
-        // the prover copies the assignments on a stream of its own: the upload must be complete before it is called
-        // (the evaluation queued below need not be -- the witness MSMs do not wait for it)
-        BB_CUDA(cudaStreamSynchronize(st));
-    }
+    DevBuf up[2], d_abc;
+    const Fr *d_in, *d_aux;
+    BB_TRY(stage_witness(ctx, st, input, n_inputs, aux, n_aux, on_device, up, &d_in, &d_aux));
+    // the prover copies the assignments on a stream of its own: the upload must be complete before it is called
+    // (the evaluation queued below need not be -- the witness MSMs do not wait for it)
+    if (!on_device) BB_CUDA(cudaStreamSynchronize(st));
     tm.mark("r1cs.upload");
     BB_TRY(d_abc.alloc(ctx, 3 * n * 32));
     Fr* oa = d_abc.as<Fr>();

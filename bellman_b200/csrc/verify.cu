@@ -146,29 +146,6 @@ __global__ void __launch_bounds__(64) k_diag_fp12(const Fp12* __restrict__ a, co
     out[i] = r;
 }
 
-// CUDA-event brackets of the stages (profile mode only)
-struct StageTimer {
-    bb_ctx* ctx;
-    cudaStream_t st;
-    std::vector<std::pair<const char*, cudaEvent_t>> marks;
-    StageTimer(bb_ctx* c, cudaStream_t s) : ctx(c), st(s) {}
-    ~StageTimer() { for (auto& m : marks) cudaEventDestroy(m.second); }
-    void mark(const char* stage_ending_here) {
-        if (!ctx->opt_profile) return;
-        cudaEvent_t e;
-        if (cudaEventCreate(&e) != cudaSuccess) return;
-        cudaEventRecord(e, st);
-        marks.emplace_back(stage_ending_here, e);
-    }
-    // after the stream has drained: stage k = the interval between marks k-1 and k
-    void report(uint64_t units) {
-        for (size_t k = 1; k < marks.size(); k++) {
-            float ms = 0;
-            if (cudaEventElapsedTime(&ms, marks[k - 1].second, marks[k].second) == cudaSuccess) ctx->prof_add(marks[k].first, ms, 1, units);
-        }
-    }
-};
-
 // Root of the batch: miller values of all pairs in d_f[0, m) -> verdict (and the G_T value, host, if asked)
 int product_and_final_exp(bb_ctx* ctx, cudaStream_t st, Fp12* d_f, size_t m, StageTimer& tm, bool* accepted, Fp12* gt_host) {
     DevBuf d_tmp, d_out;
@@ -234,16 +211,24 @@ void gt_to_canonical(const Fp12& g, void* out) {
     for (int k = 0; k < 12; k++) o[k] = fp_to_canonical(c[k]);
 }
 
-// The batch verifier.  gt_host: optional, receives the G_T value the verdict was taken from.
-int verify_batch(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* b, const void* z_in, Fp12* gt_host) {
-    if (!ctx || !vk || !b) { set_error("bb_groth16_verify_batch: null argument"); return BB_ERR_ARG; }
+// The argument checks of verify_batch and verify_each, before any device work.  outputs: the caller's output arrays
+// are present (checked with the proof arrays).
+int check_proof_batch(const char* fn, const bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* b, bool outputs) {
+    if (!ctx || !vk || !b) { set_error("%s: null argument", fn); return BB_ERR_ARG; }
     const size_t n = b->n, L = b->n_inputs;
-    if (n && (!b->a || !b->b || !b->c || (L && !b->inputs))) { set_error("bb_groth16_verify_batch: null proof array"); return BB_ERR_ARG; }
-    if (n && L + 1 != vk->ic_len) {                              // batch.rs:105-111, before any device work
+    if (n && (!outputs || !b->a || !b->b || !b->c || (L && !b->inputs))) { set_error("%s: null array", fn); return BB_ERR_ARG; }
+    if (n && L + 1 != vk->ic_len) {                              // batch.rs:105-111
         set_error("InvalidVerifyingKey: %zu public inputs for a key with %zu ic entries", L, vk->ic_len);
         return BB_ERR_INVALID_VERIFYING_KEY;
     }
-    if (n >= (1ull << 31)) { set_error("bb_groth16_verify_batch: more than 2^31 proofs"); return BB_ERR_ARG; }
+    if (n >= (1ull << 31)) { set_error("%s: more than 2^31 proofs", fn); return BB_ERR_ARG; }
+    return BB_OK;
+}
+
+// The batch verifier.  gt_host: optional, receives the G_T value the verdict was taken from.
+int verify_batch(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* b, const void* z_in, Fp12* gt_host) {
+    BB_TRY(check_proof_batch("bb_groth16_verify_batch", ctx, vk, b, true));
+    const size_t n = b->n, L = b->n_inputs;
     std::vector<Fr> z(n);
     if (z_in) {
         std::memcpy(z.data(), z_in, n * 32);
@@ -261,22 +246,14 @@ int verify_batch(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* b, const vo
     cudaStream_t st = ctx->main_stream;
     StageTimer tm(ctx, st);
     tm.mark("verify.begin");
-    const G1Affine *d_a = (const G1Affine*)b->a, *d_c = (const G1Affine*)b->c;
-    const G2Affine* d_b = (const G2Affine*)b->b;
-    const Fr* d_x = (const Fr*)b->inputs;
+    const G1Affine *d_a, *d_c;
+    const G2Affine* d_b;
+    const Fr* d_x;
     DevBuf up_a, up_b, up_c, up_x, d_z, d_zm, d_scc, d_part, d_acc, d_pe, d_q, d_f;
-    if (!b->on_device) {
-        BB_TRY(up_a.alloc(ctx, n * sizeof(G1Affine)));
-        BB_TRY(up_b.alloc(ctx, n * sizeof(G2Affine)));
-        BB_TRY(up_c.alloc(ctx, n * sizeof(G1Affine)));
-        BB_TRY(up_x.alloc(ctx, n * L * 32));
-        BB_CUDA(cudaMemcpyAsync(up_a.p, b->a, n * sizeof(G1Affine), cudaMemcpyHostToDevice, st));
-        BB_CUDA(cudaMemcpyAsync(up_b.p, b->b, n * sizeof(G2Affine), cudaMemcpyHostToDevice, st));
-        BB_CUDA(cudaMemcpyAsync(up_c.p, b->c, n * sizeof(G1Affine), cudaMemcpyHostToDevice, st));
-        if (L) BB_CUDA(cudaMemcpyAsync(up_x.p, b->inputs, n * L * 32, cudaMemcpyHostToDevice, st));
-        ctx->h2d_bytes += n * (2 * sizeof(G1Affine) + sizeof(G2Affine) + L * 32);
-        d_a = up_a.as<G1Affine>(); d_b = up_b.as<G2Affine>(); d_c = up_c.as<G1Affine>(); d_x = up_x.as<Fr>();
-    }
+    BB_TRY(device_input(ctx, st, b->a, n * sizeof(G1Affine), b->on_device, up_a, &d_a));
+    BB_TRY(device_input(ctx, st, b->b, n * sizeof(G2Affine), b->on_device, up_b, &d_b));
+    BB_TRY(device_input(ctx, st, b->c, n * sizeof(G1Affine), b->on_device, up_c, &d_c));
+    BB_TRY(device_input(ctx, st, b->inputs, n * L * 32, b->on_device, up_x, &d_x));
     const size_t pairs = n + 3, chunks = (n + COLSUM_CHUNK - 1) / COLSUM_CHUNK;
     BB_TRY(d_z.alloc(ctx, n * 32));
     BB_TRY(d_zm.alloc(ctx, n * 32));
@@ -516,17 +493,8 @@ int each_key(bb_ctx* ctx, const bb_vk* vk, const EachKey** out) {
 
 // verify_proof per proof.  gt_host: optional, n + 1 values: every proof's FE(f_i), then the target.
 int verify_each(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* b, uint8_t* verdicts, size_t* n_invalid, Fp12* gt_host) {
-    if (!ctx || !vk || !b) { set_error("bb_groth16_verify_each: null argument"); return BB_ERR_ARG; }
+    BB_TRY(check_proof_batch("bb_groth16_verify_each", ctx, vk, b, verdicts && n_invalid));
     const size_t n = b->n, L = b->n_inputs;
-    if (n && (!verdicts || !n_invalid || !b->a || !b->b || !b->c || (L && !b->inputs))) {
-        set_error("bb_groth16_verify_each: null array");
-        return BB_ERR_ARG;
-    }
-    if (n && L + 1 != vk->ic_len) {                              // before any device work, as verify_batch
-        set_error("InvalidVerifyingKey: %zu public inputs for a key with %zu ic entries", L, vk->ic_len);
-        return BB_ERR_INVALID_VERIFYING_KEY;
-    }
-    if (n >= (1ull << 31)) { set_error("bb_groth16_verify_each: more than 2^31 proofs"); return BB_ERR_ARG; }
     if (n_invalid) *n_invalid = 0;
     if (n == 0 && !gt_host) return BB_OK;
     BB_CUDA(cudaSetDevice(ctx->device));
@@ -541,22 +509,14 @@ int verify_each(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* b, uint8_t* 
     }
     StageTimer tm(ctx, st);
     tm.mark("verify_each.begin");
-    const G1Affine *d_a = (const G1Affine*)b->a, *d_c = (const G1Affine*)b->c;
-    const G2Affine* d_b = (const G2Affine*)b->b;
-    const Fr* d_x = (const Fr*)b->inputs;
+    const G1Affine *d_a, *d_c;
+    const G2Affine* d_b;
+    const Fr* d_x;
     DevBuf up_a, up_b, up_c, up_x, d_pe, d_f, d_v, d_gt;
-    if (!b->on_device) {
-        BB_TRY(up_a.alloc(ctx, n * sizeof(G1Affine)));
-        BB_TRY(up_b.alloc(ctx, n * sizeof(G2Affine)));
-        BB_TRY(up_c.alloc(ctx, n * sizeof(G1Affine)));
-        BB_TRY(up_x.alloc(ctx, n * L * 32));
-        BB_CUDA(cudaMemcpyAsync(up_a.p, b->a, n * sizeof(G1Affine), cudaMemcpyHostToDevice, st));
-        BB_CUDA(cudaMemcpyAsync(up_b.p, b->b, n * sizeof(G2Affine), cudaMemcpyHostToDevice, st));
-        BB_CUDA(cudaMemcpyAsync(up_c.p, b->c, n * sizeof(G1Affine), cudaMemcpyHostToDevice, st));
-        if (L) BB_CUDA(cudaMemcpyAsync(up_x.p, b->inputs, n * L * 32, cudaMemcpyHostToDevice, st));
-        ctx->h2d_bytes += n * (2 * sizeof(G1Affine) + sizeof(G2Affine) + L * 32);
-        d_a = up_a.as<G1Affine>(); d_b = up_b.as<G2Affine>(); d_c = up_c.as<G1Affine>(); d_x = up_x.as<Fr>();
-    }
+    BB_TRY(device_input(ctx, st, b->a, n * sizeof(G1Affine), b->on_device, up_a, &d_a));
+    BB_TRY(device_input(ctx, st, b->b, n * sizeof(G2Affine), b->on_device, up_b, &d_b));
+    BB_TRY(device_input(ctx, st, b->c, n * sizeof(G1Affine), b->on_device, up_c, &d_c));
+    BB_TRY(device_input(ctx, st, b->inputs, n * L * 32, b->on_device, up_x, &d_x));
     BB_TRY(d_pe.alloc(ctx, n * sizeof(G1Eval)));
     BB_TRY(d_f.alloc(ctx, n * sizeof(Fp12)));
     BB_TRY(d_v.alloc(ctx, n));

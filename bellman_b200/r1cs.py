@@ -15,7 +15,7 @@ import ctypes as C
 
 import numpy as np
 
-from . import EvaluationDomain, _c64, _check, _ptr, _scalar_bytes, load_library
+from . import EvaluationDomain, _addr, _c64, _check, _DeviceObject, _ptr, _scalar_bytes, load_library
 
 FR_MODULUS = EvaluationDomain.FR_MODULUS
 SHAPE_WORDS = 9
@@ -31,10 +31,6 @@ class _Desc(C.Structure):
                 ("n_constraints", C.c_size_t), ("n_inputs", C.c_size_t), ("n_aux", C.c_size_t)]
 
 
-def _addr(p):
-    return p.value if isinstance(p, C.c_void_p) else int(p)
-
-
 def _unpack(words, n):
     return np.unpackbits(np.ascontiguousarray(words, np.uint64).view(np.uint8), bitorder="little")[:n].astype(bool)
 
@@ -43,13 +39,14 @@ def _mont_limbs(ints):
     """Python integers mod r -> (n, 4) uint64 Montgomery limbs"""
     out = np.zeros((len(ints), 4), np.uint64)
     for i, v in enumerate(ints):
-        m = (v % FR_MODULUS) * (1 << 256) % FR_MODULUS
-        out[i] = [(m >> (64 * j)) & _MASK64 for j in range(4)]
+        out[i] = EvaluationDomain._to_mont(v)
     return out
 
 
-class R1CS:
+class R1CS(_DeviceObject):
     """bb_r1cs: the A, B, C matrices of one circuit in HBM.  a, b, c: (row_offsets, vars, coeffs) per matrix."""
+
+    _destroy = "bb_r1cs_destroy"
 
     def __init__(self, worker, n_inputs, n_aux, a, b, c):
         mats = []
@@ -67,13 +64,12 @@ class R1CS:
         d.n_constraints, d.n_inputs, d.n_aux = n, n_inputs, n_aux
         h = C.c_void_p()
         _check(load_library().bb_r1cs_create(worker._h, C.byref(d), C.byref(h)))
-        self.worker, self._h = worker, h
+        self._own(worker, h)
         shape = np.zeros(SHAPE_WORDS, np.uint64)
         _check(load_library().bb_r1cs_info(h, _ptr(shape), None, None, None))
         self.n_constraints, self.n_inputs, self.n_aux = (int(x) for x in shape[:3])
         self.nnz = tuple(int(x) for x in shape[3:6])              # terms the evaluation reads, per matrix
         self.unit = tuple(int(x) for x in shape[6:9])             # of those, coefficient one
-        worker._children.add(self)
 
     @classmethod
     def from_assembly(cls, worker, asm):
@@ -123,23 +119,25 @@ class R1CS:
         """a, b, c for the witness (bb_r1cs_eval).  Host arrays of Montgomery Fr, or with on_device=True device addresses
         (lengths taken from the constraint system).  out: None -> three (n, 4) host arrays returned; or a dict a, b, c
         of device addresses written in place."""
-        if on_device:
-            src = (C.c_void_p(_addr(input_assignment)), self.n_inputs, C.c_void_p(_addr(aux_assignment)), self.n_aux)
-            keep = ()
-        else:
-            inp, aux = _c64(input_assignment, 4), _c64(aux_assignment, 4)
-            src = (_ptr(inp), inp.shape[0], _ptr(aux), aux.shape[0])
-            keep = (inp, aux)
+        src, keep = self._witness_args(input_assignment, aux_assignment, on_device)
         if out is None:
             res = [np.zeros((self.n_constraints, 4), np.uint64) for _ in range(3)]
             dst = [_ptr(x) for x in res]
         else:
             res = None
             dst = [C.c_void_p(_addr(out[k])) for k in "abc"]
-        _check(load_library().bb_r1cs_eval(self.worker._h, self._h, src[0], C.c_size_t(src[1]), src[2], C.c_size_t(src[3]),
-                                           C.c_int(1 if on_device else 0), *dst, C.c_int(0 if out is None else 1)))
+        _check(load_library().bb_r1cs_eval(self.worker._h, self._h, *src, *dst, C.c_int(0 if out is None else 1)))
         del keep
         return None if res is None else tuple(res)
+
+    def _witness_args(self, input_assignment, aux_assignment, on_device):
+        """the (input, n_inputs, aux, n_aux, on_device) arguments of bb_r1cs_eval and bb_groth16_prove_r1cs, and the host
+        arrays they point into: device addresses (lengths taken from the constraint system), or host arrays"""
+        if on_device:
+            return (C.c_void_p(_addr(input_assignment)), C.c_size_t(self.n_inputs), C.c_void_p(_addr(aux_assignment)),
+                    C.c_size_t(self.n_aux), C.c_int(1)), ()
+        inp, aux = _c64(input_assignment, 4), _c64(aux_assignment, 4)
+        return (_ptr(inp), C.c_size_t(inp.shape[0]), _ptr(aux), C.c_size_t(aux.shape[0]), C.c_int(0)), (inp, aux)
 
     def assignment(self, input_assignment, aux_assignment):
         """the ProvingAssignment bellman's synthesis would have built, evaluated on the device"""
@@ -151,33 +149,16 @@ class R1CS:
         asg.a_aux_density, asg.b_input_density, asg.b_aux_density = self.density_words()
         return asg
 
-    def free(self):
-        if getattr(self, "_h", None):
-            if getattr(self.worker, "_h", None):
-                load_library().bb_r1cs_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.free()
-        except Exception:
-            pass
-
 
 def create_proof_r1cs(r1cs, params, input_assignment, aux_assignment, r, s, device_ptrs=None):
     """create_proof from the witness alone (bb_groth16_prove_r1cs): the bytes create_proof gives for the
     ProvingAssignment synthesis would have built.  device_ptrs: optional dict inputs, aux -> device addresses (the
     witness resident in HBM; input_assignment / aux_assignment are then ignored)."""
     if device_ptrs is not None:
-        src = (C.c_void_p(_addr(device_ptrs["inputs"])), r1cs.n_inputs, C.c_void_p(_addr(device_ptrs["aux"])), r1cs.n_aux, 1)
-        keep = ()
-    else:
-        inp, aux = _c64(input_assignment, 4), _c64(aux_assignment, 4)
-        src = (_ptr(inp), inp.shape[0], _ptr(aux), aux.shape[0], 0)
-        keep = (inp, aux)
+        input_assignment, aux_assignment = device_ptrs["inputs"], device_ptrs["aux"]
+    src, keep = r1cs._witness_args(input_assignment, aux_assignment, device_ptrs is not None)
     proof = (C.c_uint8 * 192)()
-    _check(load_library().bb_groth16_prove_r1cs(params.worker._h, params._h, r1cs._h, src[0], C.c_size_t(src[1]), src[2],
-                                                C.c_size_t(src[3]), C.c_int(src[4]), _scalar_bytes(r), _scalar_bytes(s), proof))
+    _check(load_library().bb_groth16_prove_r1cs(params.worker._h, params._h, r1cs._h, *src, _scalar_bytes(r), _scalar_bytes(s), proof))
     del keep
     return bytes(proof)
 

@@ -16,11 +16,12 @@ Proofs as bytes (Proof::read / Proof::write, groth16/src/lib.rs:39-99, over bb_p
     proof = read_proof(worker, b192)                           # raises InvalidProofEncoding like Proof::read
     bv.queue_bytes((b192, inputs)); bv.verify(rng, pvk)        # decoded on the device at verify() time
 """
+import contextlib
 import ctypes as C
 
 import numpy as np
 
-from . import BackendError, EvaluationDomain, _addr, _c64, _check, _ERRORS, _ptr, load_library
+from . import BackendError, EvaluationDomain, _addr, _c64, _check, _DeviceObject, _ERRORS, _ptr, load_library
 
 
 class VerificationError(Exception):
@@ -51,8 +52,10 @@ class _ProofBatch(C.Structure):
                 ("inputs", C.c_void_p), ("n_inputs", C.c_size_t), ("on_device", C.c_int)]
 
 
-class PreparedVerifyingKey:
+class PreparedVerifyingKey(_DeviceObject):
     """groth16::PreparedVerifyingKey (groth16/src/lib.rs:400-409): the key resident on the device."""
+
+    _destroy = "bb_vk_destroy"
 
     def __init__(self, worker, vk):
         self.worker = worker
@@ -65,20 +68,7 @@ class PreparedVerifyingKey:
         self.ic_len = int(d.ic_len)
         h = C.c_void_p()
         _check(load_library().bb_vk_prepare(worker._h, C.byref(d), C.byref(h)))
-        self._h = h
-        worker._children.add(self)
-
-    def free(self):
-        if getattr(self, "_h", None):
-            if getattr(self.worker, "_h", None):
-                load_library().bb_vk_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.free()
-        except Exception:
-            pass
+        self._own(worker, h)
 
 
 def prepare_verifying_key(worker, vk):
@@ -135,7 +125,7 @@ def _proof_batch(a, b, c, inputs, on_device, n, n_inputs, keep):
     """the bb_proof_batch of verify_batch_arrays' arguments, and n; host arrays are appended to keep"""
     bt = _ProofBatch()
     if on_device:
-        bt.a, bt.b, bt.c, bt.inputs = (p.value if isinstance(p, C.c_void_p) else p for p in (a, b, c, inputs))
+        bt.a, bt.b, bt.c, bt.inputs = (_addr(p) for p in (a, b, c, inputs))
         bt.n, bt.n_inputs, bt.on_device = n, n_inputs, 1
         return bt, n
     a, b, c = _c64(a, 12), _c64(b, 24), _c64(c, 12)
@@ -294,40 +284,58 @@ class BatchVerifier:
         if n and any(x.shape[0] + 1 != pvk.ic_len for _, x in self.items):
             raise InvalidVerifyingKey(f"[bb_status 6] InvalidVerifyingKey: a key with {pvk.ic_len} ic entries")
         L = pvk.ic_len - 1
-        a = np.stack([p[0].reshape(12) for p, _ in self.items]) if n else np.zeros((0, 12), np.uint64)
-        b = np.stack([p[1].reshape(24) for p, _ in self.items]) if n else np.zeros((0, 24), np.uint64)
-        c = np.stack([p[2].reshape(12) for p, _ in self.items]) if n else np.zeros((0, 12), np.uint64)
-        x = np.stack([xi.reshape(L, 4) for _, xi in self.items]) if n and L else np.zeros((n, max(L, 0), 4), np.uint64)
         z = None if rng is None else [rng.randrange(1, R_MODULUS) for _ in range(n)]
-        verify_batch_arrays(pvk, a, b, c, x, z, n_inputs=max(L, 0))
+        verify_batch_arrays(pvk, *self._points(range(n)), self._inputs(range(n), L), z, n_inputs=max(L, 0))
 
     def _verify_from_bytes(self, rng, pvk):
-        """the batch in device buffers: the queue_bytes proofs first (decoded in place), then the queue() ones (uploaded);
-        the verdict of a batch does not depend on the order of its items"""
-        worker, n, L = pvk.worker, len(self.items), pvk.ic_len - 1
-        enc = [i for i, (p, _) in enumerate(self.items) if isinstance(p, bytes)]
-        dec = [i for i, (p, _) in enumerate(self.items) if not isinstance(p, bytes)]
-        nb = len(enc)
-        d = {"a": worker.device_alloc(n * 96), "b": worker.device_alloc(n * 192), "c": worker.device_alloc(n * 96),
-             "x": worker.device_alloc(max(1, n * max(L, 0)) * 32)}
-        try:
-            _, _, _, status = read_proofs(worker, b"".join(self.items[i][0] for i in enc), n=nb, out_device=(d["a"], d["b"], d["c"]))
+        """the batch in device buffers (see _staged); the verdict of a batch does not depend on the order of its items"""
+        n, L = len(self.items), pvk.ic_len - 1
+        enc, dec = self._split()
+        with self._staged(pvk.worker, enc, dec, self._inputs(enc + dec, L)) as (d, status):
             bad = np.flatnonzero(status)
             if bad.size:
                 k = int(bad[0])
                 raise InvalidProofEncoding(f"{read_error_message(int(status[k]))} (queued proof {enc[k]})", status=int(status[k]), index=enc[k])
             if any(x.shape[0] + 1 != pvk.ic_len for _, x in self.items):
                 raise InvalidVerifyingKey(f"[bb_status 6] InvalidVerifyingKey: a key with {pvk.ic_len} ic entries")
-            if dec:
-                for key, k, width in (("a", 0, 12), ("b", 1, 24), ("c", 2, 12)):
-                    rows = np.stack([self.items[i][0][k].reshape(width) for i in dec])
-                    worker.upload(C.c_void_p(_addr(d[key]) + nb * width * 8), rows)
-            if L:
-                worker.upload(d["x"], np.stack([self.items[i][1].reshape(L, 4) for i in enc + dec]))
             z = None if rng is None else [rng.randrange(1, R_MODULUS) for _ in range(n)]
-            verify_batch_arrays(pvk, d["a"], d["b"], d["c"], d["x"], z, on_device=True, n=n, n_inputs=L)
+            verify_batch_arrays(pvk, *d, z, on_device=True, n=n, n_inputs=L)
+
+    def _split(self):
+        """the queue indices of the queue_bytes items and of the queue() items"""
+        enc = [i for i, (p, _) in enumerate(self.items) if isinstance(p, bytes)]
+        return enc, [i for i, (p, _) in enumerate(self.items) if not isinstance(p, bytes)]
+
+    def _points(self, order):
+        """the a (k, 12), b (k, 24), c (k, 12) arrays of the queue() items at the queue indices `order`"""
+        return [np.stack([self.items[i][0][k].reshape(w) for i in order]) if len(order) else np.zeros((0, w), np.uint64)
+                for k, w in ((0, 12), (1, 24), (2, 12))]
+
+    def _inputs(self, order, L):
+        """the (k, L, 4) public inputs of the items at the queue indices `order`; zero rows for items of another length"""
+        x = np.zeros((len(order), max(L, 0), 4), np.uint64)
+        for k, i in enumerate(order):
+            if self.items[i][1].shape[0] == L:
+                x[k] = self.items[i][1].reshape(L, 4)
+        return x
+
+    @contextlib.contextmanager
+    def _staged(self, worker, enc, dec, x):
+        """the queue in device buffers a, b, c, x, freed on exit: the queue_bytes items `enc` decoded in place by one
+        read_proofs, the queue() items `dec` uploaded behind them, and the inputs x (rows in the order enc + dec).
+        Yields the four buffers and the status bytes of the enc items."""
+        n, nb = len(enc) + len(dec), len(enc)
+        d = [worker.device_alloc(n * 96), worker.device_alloc(n * 192), worker.device_alloc(n * 96), worker.device_alloc(max(1, x.size // 4) * 32)]
+        try:
+            _, _, _, status = read_proofs(worker, b"".join(self.items[i][0] for i in enc), n=nb, out_device=d[:3])
+            if dec:
+                for buf, rows in zip(d, self._points(dec)):
+                    worker.upload(C.c_void_p(_addr(buf) + nb * rows.shape[1] * 8), rows)
+            if x.size:
+                worker.upload(d[3], x)
+            yield d, status
         finally:
-            for p in d.values():
+            for p in d:
                 worker.device_free(p)
 
     def verify_each(self, pvk):
@@ -337,7 +345,7 @@ class BatchVerifier:
         of inputs (the other items are still verified); InvalidProofEncoding (with its queue index) for a queue_bytes item
         that does not read.  The queue_bytes items are decoded in one bb_proofs_read into device buffers and verified
         there.  Only back-end failures raise."""
-        worker, n, L = pvk.worker, len(self.items), pvk.ic_len - 1
+        n, L = len(self.items), pvk.ic_len - 1
         out = [None] * n
         for i, (_, x) in enumerate(self.items):
             if x.shape[0] != L:
@@ -345,35 +353,17 @@ class BatchVerifier:
                                              f"{pvk.ic_len} ic entries (queued item {i})")
         if n == 0 or L < 0:
             return out
-        enc = [i for i, (p, _) in enumerate(self.items) if isinstance(p, bytes)]
-        dec = [i for i, (p, _) in enumerate(self.items) if not isinstance(p, bytes)]
+        enc, dec = self._split()
         order = enc + dec                                       # device row k holds queue item order[k]
-        x = np.zeros((n, L, 4), np.uint64)                      # zero rows for the items of a wrong input count
-        for k, i in enumerate(order):
-            if out[i] is None and L:
-                x[k] = self.items[i][1].reshape(L, 4)
+        x = self._inputs(order, L)                              # zero rows for the items of a wrong input count
         if not enc:
-            pts = [np.stack([self.items[i][0][k].reshape(w) for i in order]) for k, w in ((0, 12), (1, 24), (2, 12))]
-            verdicts = verify_each_arrays(pvk, *pts, x, n_inputs=L)
+            verdicts = verify_each_arrays(pvk, *self._points(order), x, n_inputs=L)
         else:
-            nb = len(enc)
-            d = {"a": worker.device_alloc(n * 96), "b": worker.device_alloc(n * 192), "c": worker.device_alloc(n * 96),
-                 "x": worker.device_alloc(max(1, n * L) * 32)}
-            try:
-                _, _, _, status = read_proofs(worker, b"".join(self.items[i][0] for i in enc), n=nb, out_device=(d["a"], d["b"], d["c"]))
+            with self._staged(pvk.worker, enc, dec, x) as (d, status):
                 for k, i in enumerate(enc):                     # Proof::read fails before the item could be queued
                     if status[k]:
                         out[i] = InvalidProofEncoding(f"{read_error_message(int(status[k]))} (queued proof {i})", status=int(status[k]), index=i)
-                if dec:
-                    for key, k, width in (("a", 0, 12), ("b", 1, 24), ("c", 2, 12)):
-                        rows = np.stack([self.items[i][0][k].reshape(width) for i in dec])
-                        worker.upload(C.c_void_p(_addr(d[key]) + nb * width * 8), rows)
-                if L:
-                    worker.upload(d["x"], x)
-                verdicts = verify_each_arrays(pvk, d["a"], d["b"], d["c"], d["x"], on_device=True, n=n, n_inputs=L)
-            finally:
-                for p in d.values():
-                    worker.device_free(p)
+                verdicts = verify_each_arrays(pvk, *d, on_device=True, n=n, n_inputs=L)
         for k, i in enumerate(order):
             if out[i] is None and verdicts[k]:
                 out[i] = InvalidProof(f"[bb_status 7] InvalidProof: queued item {i} does not verify")
