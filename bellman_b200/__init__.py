@@ -623,6 +623,61 @@ def create_random_proof(assignment, params, rng=None, device_ptrs=None):
     return create_proof(assignment, params, draw(q), draw(q), device_ptrs)
 
 
+def _batch_result(params, rc, proofs, status):
+    """one entry per item: its 192 proof bytes, or the exception create_proof raises for it alone"""
+    _check(rc)
+    raw = bytes(proofs)
+    out = []
+    for i, st in enumerate(status):
+        if st == BB_OK:
+            out.append(raw[192 * i:192 * (i + 1)])
+        else:
+            out.append(_ERRORS.get(st, BackendError)(f"[bb_status {st}] {_status_message(params, st)}"))
+    return out
+
+
+def _status_message(params, st):
+    """the message bb_groth16_prove reports with status `st` for this key (bb_groth16_prove_message); a back-end failure
+    of a sub-batch keeps the call's bb_last_error"""
+    lib = load_library()
+    lib.bb_groth16_prove_message.restype = C.c_char_p
+    msg = lib.bb_groth16_prove_message(params._h, C.c_int(st))
+    return (msg if msg is not None else lib.bb_last_error()).decode(errors="replace")
+
+
+def _scalars_bytes(vals):
+    return (C.c_uint8 * (32 * len(vals))).from_buffer_copy(b"".join(int(v).to_bytes(32, "little") for v in vals))
+
+
+def create_proof_batch(assignments, params, rs, ss, device_ptrs=None):
+    """bb_groth16_prove_batch: create_proof for every assignment of one circuit against `params`, in one call.
+    `device_ptrs`: None, or one dict per item as create_proof takes it.  Returns one entry per item: the 192 bytes
+    create_proof returns for it alone, or the exception it would raise (an instance, not raised)."""
+    n = len(assignments)
+    if not (len(rs) == len(ss) == n) or (device_ptrs is not None and len(device_ptrs) != n):
+        raise ValueError("create_proof_batch: one r, one s (and one device_ptrs entry) per assignment")
+    ws = (_Witness * max(n, 1))()
+    for i, asg in enumerate(assignments):
+        ws[i] = asg._struct(None if device_ptrs is None else device_ptrs[i])
+    proofs = (C.c_uint8 * (192 * max(n, 1)))()
+    status = (C.c_int * max(n, 1))()
+    rc = load_library().bb_groth16_prove_batch(params.worker._h, params._h, ws, C.c_size_t(n), _scalars_bytes(rs), _scalars_bytes(ss),
+                                               proofs, status)
+    return _batch_result(params, rc, proofs, list(status)[:n])
+
+
+def create_random_proof_batch(assignments, params, rng=None, device_ptrs=None):
+    """create_random_proof for every assignment: fresh (r, s) per item, then create_proof_batch"""
+    import secrets
+    draw = rng.randrange if rng is not None else secrets.randbelow
+    q = EvaluationDomain.FR_MODULUS
+    rs, ss = [], []
+    for _ in assignments:
+        rs.append(draw(q))
+        ss.append(draw(q))
+    return create_proof_batch(assignments, params, rs, ss, device_ptrs)
+
+
 def synth_mimc(rounds, seed, pinned=False):
     """bench-only: the MiMC-chain witness of `rounds` rounds as a ProvingAssignment (product-side
     generator, bellman_b200/csrc/synth.cu).  pinned=True places the arrays in page-locked host
@@ -675,4 +730,5 @@ from .verifier import (BatchVerifier, InvalidProof, InvalidVerifyingKey, Prepare
 # Proof::read / Proof::write over a batch (groth16/src/lib.rs:39-99)
 from .verifier import InvalidProofEncoding, read_proof, read_proofs, write_proofs  # noqa: E402
 # the constraint system on the device: prove from the witness alone (groth16/src/prover.rs:19-55,105-145)
-from .r1cs import R1CS, create_proof_r1cs, create_random_proof_r1cs  # noqa: E402
+from .r1cs import (R1CS, create_proof_r1cs, create_proof_r1cs_batch, create_random_proof_r1cs,  # noqa: E402
+                   create_random_proof_r1cs_batch)

@@ -5,6 +5,7 @@
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
+#include <functional>
 #include <map>
 #include <mutex>
 #include <string>
@@ -85,6 +86,7 @@ struct bb_ctx {
                                      // 1 = one bucket array per window slot, 2 = ONE bucket array for all windows
     long opt_msm_precompute_groups = 3;  // which groups use the tables: bit 0 = G1 vectors, bit 1 = G2 vectors
     long opt_msm_unified_rows_log = 3;   // msm_precompute = 2: halving rounds until about 2^this rows per bucket are left
+    long opt_prove_batch_max = 0;        // bb_groth16_prove_batch: at most this many proofs per sub-batch (0 = by memory)
     struct ProfEntry { double ms = 0; uint64_t launches = 0, units = 0; };
     std::map<std::string, ProfEntry> prof;
     void prof_add(const char* what, double ms, uint64_t launches, uint64_t units) {
@@ -179,11 +181,22 @@ inline unsigned cdiv(size_t a, size_t b) { return (unsigned)((a + b - 1) / b); }
 // ---- ntt.cu ----
 int ntt_run_device(bb_ctx* ctx, cudaStream_t st, Fr* d_data, Fr* d_tmp, uint32_t log_n, int mode);
 int h_poly_device(bb_ctx* ctx, cudaStream_t st, Fr* d_a, Fr* d_b, Fr* d_c, Fr* d_tmp, uint32_t log_m);
+int h_poly_batch_device(bb_ctx* ctx, cudaStream_t st, Fr* d_abc, Fr* d_tmp, uint32_t log_m, uint32_t B);
 int h_poly_evals_device(bb_ctx* ctx, cudaStream_t st, Fr* d_p, Fr* d_tmp, uint32_t log_m);
 int h_poly_final_device(bb_ctx* ctx, cudaStream_t st, Fr* d_a, const Fr* d_b, const Fr* d_c, Fr* d_tmp, uint32_t log_m);
 int fr_convert_device(bb_ctx* ctx, cudaStream_t st, Fr* d_data, size_t n, bool to_montgomery);
 void ntt_free_tables(bb_ctx* ctx);
 int domain_pointwise_device(bb_ctx* ctx, cudaStream_t st, Fr* d_a, const Fr* d_b, size_t n, int op, const Fr& k);
+
+// ---- prover.cu ----
+// Queues on `st` the evaluation of a sub-batch's a, b, c into abc (rows a_0 .. a_{B-1}, b_0 .., c_0 .. of m Fr; the first
+// n_constraints of each) from its uploaded witnesses d_in (B x n_inputs) and d_aux (B x n_aux)
+using BatchAbcFill = std::function<int(cudaStream_t st, uint32_t B, Fr* abc, size_t m, const Fr* d_in, const Fr* d_aux)>;
+// bb_groth16_prove_batch (with `fill`, the witnesses' a, b, c are not read: fill computes them) and its argument checks
+int prove_batch_impl(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t count, const uint8_t* r, const uint8_t* s,
+                     uint8_t* proofs, int* status, const BatchAbcFill* fill = nullptr);
+int prove_batch_check(const char* fn, const bb_ctx* ctx, const bb_crs* crs, size_t count, const void* r, const void* s, const void* proofs,
+                      const int* status);
 
 // ---- capi.cu ----
 int fixed_base_mul_device(bb_ctx* ctx, int group, const Fr* d_scalars, size_t n, bool montgomery, void* d_out, cudaStream_t st);
@@ -197,8 +210,12 @@ struct MsmResult {
 };
 int msm_start(bb_ctx* ctx, const bb_bases* bases, size_t base_offset, const uint64_t* density_bits, size_t density_len,
               const void* scalars, bool scalars_on_device, size_t n, int form, cudaEvent_t wait_for, bb_msm_job** out,
-              const char* tag = nullptr, int critical = 0);
+              const char* tag = nullptr, int critical = 0, uint32_t batch = 0, size_t scalar_stride = 0);
 int msm_wait_result(bb_msm_job* job, MsmResult* res);
+// batch != 0: one job over `batch` scalar vectors (device memory, vector p at scalars + p * scalar_stride) sharing the
+// bases, the offset and the density map; msm_wait_batch gives each vector's status and folded point
+int msm_wait_batch(bb_msm_job* job, int* status, void* points);
+size_t msm_batch_bytes(bb_ctx* ctx, const bb_bases* bases, size_t n, size_t n_dense, uint32_t batch, uint64_t* slots);
 int bases_build_table(bb_ctx* ctx, bb_bases* bases);
 // vals[i] <- 1 / vals[i] for n NON-ZERO field elements in HBM (Montgomery's trick, fan-in 32, one Fermat inversion);
 // scratch: batch_invert_scratch(n) elements

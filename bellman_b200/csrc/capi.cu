@@ -293,6 +293,7 @@ int bb_ctx_set_option(bb_ctx* ctx, const char* key, long value) {
     else if (k == "msm_precompute") { if (value < 0 || value > 2) { set_error("msm_precompute is 0, 1 or 2"); return BB_ERR_ARG; } ctx->opt_msm_precompute = value; }
     else if (k == "msm_precompute_groups") { if (value < 0 || value > 3) { set_error("msm_precompute_groups is a mask of 1 (G1) and 2 (G2)"); return BB_ERR_ARG; } ctx->opt_msm_precompute_groups = value; }
     else if (k == "msm_unified_rows_log") { if (value < 0 || value > 12) { set_error("msm_unified_rows_log is 0..12"); return BB_ERR_ARG; } ctx->opt_msm_unified_rows_log = value; }
+    else if (k == "prove_batch_max") { if (value < 0) { set_error("prove_batch_max >= 0"); return BB_ERR_ARG; } ctx->opt_prove_batch_max = value; }
     else if (k == "msm_affine_rounds") ctx->opt_msm_affine_rounds = value;
     else if (k == "msm_affine_batch") ctx->opt_msm_affine_batch = value;
     else if (k == "msm_affine_tma") ctx->opt_msm_affine_tma = value;

@@ -54,6 +54,16 @@ struct DigitArgs {
     uint32_t* err;                  // [0] = min scalar index hitting EOF (0xffffffff none), [1] identity base hit,
                                     // [4] scalars that enter the buckets here, [5] bucket entries (digits) -- profile counters
     int mode;
+    // a job over B scalar vectors (grid y = proof; one base vector, offset and density map for all of them): vector p
+    // starts at scalars + p * scalar_stride and owns the buckets [p * proof_keys, (p + 1) * proof_keys).  With proof_err
+    // set, a scalar equal to one is digit 1 of window 0 (no ones list) and an identity base under a non-zero scalar is
+    // flagged in proof_err[p] (points: the base vector, point_u4 16-byte words per point).  B = 1 without proof_err is
+    // the single job.
+    size_t scalar_stride;
+    uint32_t proof_keys;
+    uint32_t* proof_err;
+    const uint4* points;
+    uint32_t point_u4;
 };
 
 __device__ __forceinline__ uint32_t extract_bits(const uint32_t* l, uint32_t pos, uint32_t c) {
@@ -66,6 +76,7 @@ __device__ __forceinline__ uint32_t extract_bits(const uint32_t* l, uint32_t pos
 
 __global__ void __launch_bounds__(256) k_msm_digits(DigitArgs A) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t proof = blockIdx.y;
     if (i >= A.n) return;
     uint64_t rank = i;
     if (A.density) {
@@ -79,7 +90,7 @@ __global__ void __launch_bounds__(256) k_msm_digits(DigitArgs A) {
         return;
     }
     if (gi < A.shard_lo || gi >= A.shard_lo + A.shard_n) return;     // another device's shard: its scalar is never read here
-    const uint4* q = reinterpret_cast<const uint4*>(A.scalars + i);
+    const uint4* q = reinterpret_cast<const uint4*>(A.scalars + (size_t)proof * A.scalar_stride + i);
     uint4 lo = q[0], hi = q[1];
     Fr s;
     s.l[0] = lo.x; s.l[1] = lo.y; s.l[2] = lo.z; s.l[3] = lo.w;
@@ -88,7 +99,14 @@ __global__ void __launch_bounds__(256) k_msm_digits(DigitArgs A) {
     if (s.is_zero()) return;                                         // Exponent::Zero, :245
     uint32_t local = (uint32_t)(gi - A.shard_lo);
     uint32_t rest = s.l[1] | s.l[2] | s.l[3] | s.l[4] | s.l[5] | s.l[6] | s.l[7];
-    if (rest == 0 && s.l[0] == 1) {                                  // Exponent::One, :246-252
+    if (A.proof_err) {                                               // batch: the base is read under every non-zero scalar
+        if (A.mode == 0) {
+            const uint4* pt = A.points + (size_t)local * A.point_u4;
+            uint32_t any = 0;
+            for (uint32_t k = 0; k < A.point_u4; k++) { const uint4 v = pt[k]; any |= v.x | v.y | v.z | v.w; }
+            if (!any) atomicOr(&A.proof_err[proof], 1u);             // Source::next, multiexp.rs:63-65
+        }
+    } else if (rest == 0 && s.l[0] == 1) {                           // Exponent::One, :246-252
         if (A.mode == 1 && A.win_index == 0) A.ones_list[atomicAdd(A.ones_count, 1u)] = local;   // window 0's owner
         return;
     }
@@ -105,7 +123,7 @@ __global__ void __launch_bounds__(256) k_msm_digits(DigitArgs A) {
         else { mag = raw; neg = 0; carry = 0; }
         if (mag == 0 || w % A.win_count != A.win_index) continue;   // the carry chain runs over all windows
         const uint32_t slot = w / A.win_count;
-        uint32_t key = slot * A.key_stride + (mag - 1);
+        uint32_t key = proof * A.proof_keys + slot * A.key_stride + (mag - 1);
         if (A.mode == 0) atomicAdd(&A.counts[key], 1u);
         else A.sorted[atomicAdd(&A.counts[key], 1u)] = (local + slot * A.table_stride) | (neg << 31);
     }
@@ -494,14 +512,31 @@ __global__ void __launch_bounds__(128) k_table_normalize(const XYZZ<F>* __restri
         st_words(dst, a);
     }
 }
-// buckets[0][d] += buckets[1][d] + ... + buckets[slots-1][d]
+// out[p][d] = buckets[p][0][d] + buckets[p][1][d] + ... + buckets[p][slots-1][d]  (p = blockIdx.y; out may be buckets
+// itself when there is one proof)
 template <class F>
-__global__ void __launch_bounds__(128) k_msm_fold_slots(XYZZ<F>* buckets, uint32_t slots, uint32_t D) {
+__global__ void __launch_bounds__(128) k_msm_fold_slots(const XYZZ<F>* buckets, uint32_t slots, uint32_t D, XYZZ<F>* out) {
     uint32_t d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= D) return;
-    XYZZ<F> acc = ld_words(buckets + d);
-    for (uint32_t s = 1; s < slots; s++) acc.add(ld_words(buckets + (size_t)s * D + d));
-    st_words(buckets + d, acc);
+    const XYZZ<F>* in = buckets + (size_t)blockIdx.y * slots * D;
+    XYZZ<F> acc = ld_words(in + d);
+    for (uint32_t s = 1; s < slots; s++) acc.add(ld_words(in + (size_t)s * D + d));
+    st_words(out + (size_t)blockIdx.y * D + d, acc);
+}
+
+// Horner fold of each proof's W window sums (multiexp.rs:295-300) on the device: out[p] = sum_w 2^(c w) win[p * W + w].
+// One thread per proof vector of a batched job; only these B points cross the bus.
+template <class F>
+__global__ void __launch_bounds__(32) k_msm_fold_windows(const XYZZ<F>* win, uint32_t B, uint32_t W, uint32_t c, XYZZ<F>* out) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= B) return;
+    const XYZZ<F>* w = win + (size_t)p * W;
+    XYZZ<F> acc = ld_words(w + W - 1);
+    for (int k = (int)W - 2; k >= 0; k--) {
+        for (uint32_t d = 0; d < c; d++) acc = acc.dbl();
+        acc.add(ld_words(w + k));
+    }
+    st_words(out + p, acc);
 }
 
 // Error classification when BOTH an EOF and an identity base were seen: the reference folds
@@ -551,10 +586,12 @@ struct bb_msm_job {
     uint32_t affine_rounds = 0;      // batched-affine halving rounds before the XYZZ stage
     size_t n = 0;
     size_t n_dense = 0;              // scalars the density map selects (= n for FullDensity): what can reach the buckets
+    uint32_t B = 1;                  // scalar vectors (proofs) of a batched job
+    bool batched = false;            // per-proof error words and a device fold: h_out = [B points][err 8 words][B words]
     int status = BB_OK;              // pre-launch failure, reported at wait()
     const char* tag = nullptr;       // profile mode: name of this job in the prover's timeline
     DigitArgs dargs{};
-    DevBuf d_scalars, d_density, d_rank, d_counts, d_offsets, d_tiles, d_sorted, d_order, d_buckets, d_partials, d_runs, d_levels, d_onesp, d_final, d_ones, d_err, d_big, d_tasks, d_biglist, d_tasksums, d_aff0, d_aff1, d_pre, d_tp, d_doffsets, d_fold;
+    DevBuf d_scalars, d_density, d_rank, d_counts, d_offsets, d_tiles, d_sorted, d_order, d_buckets, d_partials, d_runs, d_levels, d_onesp, d_final, d_ones, d_err, d_big, d_tasks, d_biglist, d_tasksums, d_aff0, d_aff1, d_pre, d_tp, d_doffsets, d_fold, d_slotsum, d_perr, d_folded;
     std::vector<uint32_t> h_rank;
     void* h_out = nullptr;           // pinned: [W window sums][1 ones sum] then err[4]
     size_t h_out_bytes = 0;
@@ -914,20 +951,44 @@ uint32_t choose_affine_rounds(const bb_ctx* ctx, size_t pairs, uint64_t entries,
     return 0;
 }
 
+// The form, window and bucket layout of a job over B vectors of n scalars (n_dense selected by the density map): what
+// msm_start and launch_msm run, and what msm_batch_bytes estimates.  table_on_use: count a table that msm_start would
+// build on first use as present.
+struct MsmPlan { bool precomp, unified; uint32_t c, W, W_local, D, Wb, R; uint64_t NB, slots; };
+MsmPlan msm_plan(bb_ctx* ctx, const bb_bases* bases, bool table_on_use, size_t n, size_t n_dense, uint32_t B) {
+    MsmPlan p{};
+    const bool tables_wanted = ctx->opt_msm_precompute && (ctx->opt_msm_precompute_groups & (bases->group == BB_G1 ? 1 : 2));
+    const bool table = bases->d_table != nullptr || (table_on_use && tables_wanted && bases->n);
+    p.precomp = table && (tables_wanted || !ctx->opt_msm_precompute);   // a table built by hand (bb_bases_precompute) is used as it is
+    p.unified = p.precomp && ctx->opt_msm_precompute >= 2;
+    p.c = p.precomp ? (bases->d_table ? bases->tab_c : choose_window(ctx, bases->n)) : choose_window(ctx, n < bases->n + 1 ? n : bases->n + 1);
+    p.W = 255 / p.c + 1;
+    p.D = 1u << (p.c - 1);
+    const uint32_t wc = bases->win_count ? bases->win_count : 1;
+    for (uint32_t w = 0; w < p.W; w++) p.W_local += (w % wc == bases->win_index);
+    if (p.W_local == 0) p.W_local = 1;          // degenerate: more shards than windows; slot stays empty
+    p.Wb = p.unified ? 1u : p.W_local;
+    p.NB = (uint64_t)B * p.Wb * p.D;
+    p.R = p.precomp && !p.unified ? 0u : choose_affine_rounds(ctx, n_dense * B, (uint64_t)n_dense * p.W_local * B, p.NB, p.unified);
+    p.slots = (uint64_t)n * p.W_local * B + p.NB * ((1u << p.R) - 1u);
+    return p;
+}
+
 template <class F>
 int launch_msm(bb_msm_job* job) {
     NvtxRange range(job->tag ? job->tag : "bb: msm job");
     bb_ctx* ctx = job->ctx;
     cudaStream_t st = job->st;
+    const MsmPlan plan = msm_plan(ctx, job->bases, false, job->n, job->n_dense, job->B);
     const uint32_t W = job->W_local, D = job->D;   // everything below works on the owned windows only
-    const uint32_t Wb = job->unified ? 1u : W;      // bucket sets: one per window, or one for all of them
-    const size_t NB = (size_t)Wb * D;
+    const uint32_t Wb = plan.Wb;                    // bucket sets: one per window, or one for all of them
+    const uint32_t B = job->B;                      // proofs: B consecutive groups of Wb bucket sets
+    const size_t NB = plan.NB;
     const size_t n = job->n;
-    const uint64_t entries = (uint64_t)n * W;       // upper bound of the bucket entries (one per non-zero digit)
-    const uint32_t R = job->precomp && !job->unified ? 0u : choose_affine_rounds(ctx, job->n_dense, (uint64_t)job->n_dense * W, NB, job->unified);
+    const uint32_t R = plan.R;                      // halving rounds; every bucket is padded to 2^R entries
     const uint32_t pad_mask = (1u << R) - 1u;
-    const uint64_t slots = entries + (uint64_t)NB * pad_mask;   // sorted-array capacity with every bucket padded to 2^R
-    if (slots >= (1ull << 32)) { set_error("bb_msm: %zu scalars x %u windows exceed 2^32 bucket entries; split the job", n, W); return BB_ERR_ARG; }
+    const uint64_t slots = plan.slots;              // one entry per non-zero digit at most, plus the padding
+    if (slots >= (1ull << 32)) { set_error("bb_msm: %u x %zu scalars x %u windows exceed 2^32 bucket entries; split the job", B, n, W); return BB_ERR_ARG; }
     job->affine_rounds = R;
     BB_TRY(job->d_counts.alloc(ctx, (NB + 1) * 4));
     BB_TRY(job->d_offsets.alloc(ctx, (NB + 1) * 4));
@@ -939,13 +1000,15 @@ int launch_msm(bb_msm_job* job) {
     BB_TRY(job->d_buckets.alloc(ctx, NB * sizeof(XYZZ<F>)));
     BB_TRY(job->d_order.alloc(ctx, (NB + SIZE_BINS) * 4));
     const uint32_t ONES_BLOCKS = 64;
-    BB_TRY(job->d_final.alloc(ctx, (size_t)(Wb + 1) * sizeof(XYZZ<F>) + 16));
+    BB_TRY(job->d_final.alloc(ctx, ((size_t)B * Wb + 1) * sizeof(XYZZ<F>) + 16));
+    if (job->batched) BB_TRY(job->d_perr.alloc(ctx, (size_t)B * 4));
 
     BB_CUDA(cudaMemsetAsync(job->d_counts.p, 0, (NB + 1) * 4, st));
     BB_CUDA(cudaMemsetAsync(job->d_err.p, 0xff, 4, st));
     BB_CUDA(cudaMemsetAsync((char*)job->d_err.p + 4, 0, 28, st));
     BB_CUDA(cudaMemsetAsync(job->d_ones.p, 0, 4, st));
     if (R) BB_CUDA(cudaMemsetAsync(job->d_sorted.p, 0xff, slots * 4, st));      // AFF_NULL padding
+    if (job->batched) BB_CUDA(cudaMemsetAsync(job->d_perr.p, 0, (size_t)B * 4, st));
 
     const bool prof = ctx->opt_profile != 0;
     if (prof) {
@@ -958,10 +1021,14 @@ int launch_msm(bb_msm_job* job) {
     A.ones_count = job->d_ones.as<uint32_t>();
     A.ones_list = job->d_ones.as<uint32_t>() + 4;
     A.err = job->d_err.as<uint32_t>();
+    A.proof_keys = (uint32_t)((size_t)Wb * D);
+    A.proof_err = job->batched ? job->d_perr.as<uint32_t>() : nullptr;
+    A.points = (const uint4*)job->bases->d_points;
+    A.point_u4 = (uint32_t)(sizeof(Affine<F>) / 16);
     BB_STAGE("setup");
     if (n) {
         A.mode = 0;
-        k_msm_digits<<<cdiv(n, 256), 256, 0, st>>>(A);
+        k_msm_digits<<<dim3(cdiv(n, 256), B), 256, 0, st>>>(A);
         ctx->count_launch();
     }
     BB_STAGE("histogram");
@@ -974,7 +1041,7 @@ int launch_msm(bb_msm_job* job) {
     BB_STAGE("scan");
     if (n) {
         A.mode = 1;
-        k_msm_digits<<<cdiv(n, 256), 256, 0, st>>>(A);
+        k_msm_digits<<<dim3(cdiv(n, 256), B), 256, 0, st>>>(A);
         ctx->count_launch();
     }
     BB_STAGE("scatter");
@@ -1076,29 +1143,46 @@ int launch_msm(bb_msm_job* job) {
     if (prof) BB_CUDA(cudaEventRecord(job->ev[2], st));
     BB_STAGE("accumulate");
     XYZZ<F>* fin = job->d_final.as<XYZZ<F>>();
-    uint32_t Wr = Wb;                                  // window sums the reduction produces
+    uint32_t Wr = Wb;                                  // window sums the reduction produces (per proof)
     if (job->precomp && !job->unified) {
-        if (W > 1) { k_msm_fold_slots<F><<<cdiv(D, 128), 128, 0, st>>>(buckets, W, D); ctx->count_launch(); }
+        if (W > 1) {
+            XYZZ<F>* folded = buckets;                 // one proof: in place; several: each proof's D sums side by side
+            if (B > 1) { BB_TRY(job->d_slotsum.alloc(ctx, (size_t)B * D * sizeof(XYZZ<F>))); folded = job->d_slotsum.as<XYZZ<F>>(); }
+            k_msm_fold_slots<F><<<dim3(cdiv(D, 128), B), 128, 0, st>>>(buckets, W, D, folded);
+            ctx->count_launch();
+            buckets = folded;
+        }
         Wr = 1;
         BB_STAGE("fold slots");
     }
     job->W_out = Wr;
-    BB_TRY(reduce_buckets_2d<F>(ctx, st, buckets, Wr, D, (uint32_t)ctx->opt_msm_reduce_k, (uint32_t)ctx->opt_msm_reduce_k1, job->d_fold, job->d_runs, job->d_partials, job->d_levels, fin));
+    BB_TRY(reduce_buckets_2d<F>(ctx, st, buckets, B * Wr, D, (uint32_t)ctx->opt_msm_reduce_k, (uint32_t)ctx->opt_msm_reduce_k1, job->d_fold, job->d_runs, job->d_partials, job->d_levels, fin));
     size_t sh = 128 * sizeof(XYZZ<F>);
     if (sh > 48 * 1024) BB_CUDA(cudaFuncSetAttribute(k_msm_sum_list<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
     BB_TRY(job->d_onesp.alloc(ctx, ONES_BLOCKS * sizeof(XYZZ<F>)));
     XYZZ<F>* ones_partials = job->d_onesp.as<XYZZ<F>>();
     k_msm_sum_list<F><<<ONES_BLOCKS, 128, sh, st>>>(bases, A.ones_list, A.ones_count, ones_partials, A.err);
-    k_point_tree_sum<F><<<1, 128, sh, st>>>(ones_partials, ONES_BLOCKS, fin + Wr);
+    k_point_tree_sum<F><<<1, 128, sh, st>>>(ones_partials, ONES_BLOCKS, fin + (size_t)B * Wr);
     ctx->count_launch(2);
     BB_STAGE("reduce");
-    BB_CUDA(cudaGetLastError());
+    const XYZZ<F>* result = fin;
     size_t pts = (size_t)(Wr + 1) * sizeof(XYZZ<F>);
-    job->h_out_bytes = pts + 32;
+    if (job->batched) {                                // the ones are in the buckets: one folded point per proof
+        BB_TRY(job->d_folded.alloc(ctx, (size_t)B * sizeof(XYZZ<F>)));
+        k_msm_fold_windows<F><<<cdiv(B, 32), 32, 0, st>>>(fin, B, Wr, job->c, job->d_folded.as<XYZZ<F>>());
+        ctx->count_launch();
+        result = job->d_folded.as<XYZZ<F>>();
+        pts = (size_t)B * sizeof(XYZZ<F>);
+        BB_STAGE("fold windows");
+    }
+    BB_CUDA(cudaGetLastError());
+    const size_t perr = job->batched ? (size_t)B * 4 : 0;
+    job->h_out_bytes = pts + 32 + perr;
     BB_TRY(ctx->pinned_acquire(job->h_out_bytes, &job->h_out));
-    BB_CUDA(cudaMemcpyAsync(job->h_out, fin, pts, cudaMemcpyDeviceToHost, st));
+    BB_CUDA(cudaMemcpyAsync(job->h_out, result, pts, cudaMemcpyDeviceToHost, st));
     BB_CUDA(cudaMemcpyAsync((char*)job->h_out + pts, job->d_err.p, 32, cudaMemcpyDeviceToHost, st));
-    ctx->d2h_bytes += pts + 32;
+    if (perr) BB_CUDA(cudaMemcpyAsync((char*)job->h_out + pts + 32, job->d_perr.p, perr, cudaMemcpyDeviceToHost, st));
+    ctx->d2h_bytes += pts + 32 + perr;
     if (prof) BB_CUDA(cudaEventRecord(job->ev[3], st));
     // a proof has eight of these waits on eight host threads, and a multi-GPU box one process per GPU: the waiters
     // must not burn a core each (cudaStreamSynchronize spins by default)
@@ -1161,8 +1245,9 @@ int bases_build_table(bb_ctx* ctx, bb_bases* b) {
 namespace bb {
 int msm_start(bb_ctx* ctx, const bb_bases* bases, size_t base_offset, const uint64_t* density_bits, size_t density_len,
               const void* scalars, bool scalars_on_device, size_t n, int form, cudaEvent_t wait_for, bb_msm_job** out,
-              const char* tag, int critical) {
+              const char* tag, int critical, uint32_t batch, size_t scalar_stride) {
     if (!ctx || !bases || !out || (n && !scalars)) { set_error("bb_msm: null argument"); return BB_ERR_ARG; }
+    if (batch && (!scalars_on_device || bases->win_count > 1 || batch > 65535)) { set_error("bb_msm: a batched job takes device scalars, an unsharded vector and at most 65535 proofs"); return BB_ERR_ARG; }
     if (n >= (1ull << 31) || bases->n >= (1ull << 31)) { set_error("bb_msm: more than 2^31 terms"); return BB_ERR_ARG; }
     if (form != BB_FORM_CANONICAL && form != BB_FORM_MONTGOMERY) { set_error("bb_msm: bad form"); return BB_ERR_ARG; }
     BB_CUDA(cudaSetDevice(ctx->device));
@@ -1170,6 +1255,7 @@ int msm_start(bb_ctx* ctx, const bb_bases* bases, size_t base_offset, const uint
     *out = job;
     job->ctx = ctx; job->bases = bases; job->group = bases->group; job->n = n; job->n_dense = n;
     job->tag = tag;
+    job->B = batch ? batch : 1; job->batched = batch != 0;
     job->st = critical ? ctx->crit_stream[(critical - 1) & 1] : ctx->pick_stream();
     if (wait_for) BB_CUDA(cudaStreamWaitEvent(job->st, wait_for, 0));
     if (density_bits && density_len != n) {                 // the assert! at multiexp.rs:324-329
@@ -1185,14 +1271,16 @@ int msm_start(bb_ctx* ctx, const bb_bases* bases, size_t base_offset, const uint
         // of a window-sharded key must all cut the scalars into the same windows
         if (ts != BB_OK && !(ts == BB_ERR_OOM && bases->win_count <= 1)) { job->status = ts; return BB_OK; }
     }
-    job->precomp = bases->d_table != nullptr && (tables_wanted || !ctx->opt_msm_precompute);   // a table built by hand (bb_bases_precompute) is used as it is
-    job->unified = job->precomp && ctx->opt_msm_precompute >= 2;
-    job->c = job->precomp ? bases->tab_c : choose_window(ctx, n < bases->n + 1 ? n : bases->n + 1);
-    job->W = 255 / job->c + 1;
-    job->D = 1u << (job->c - 1);
+    const MsmPlan plan = msm_plan(ctx, bases, false, n, n, job->B);
+    job->precomp = plan.precomp;
+    job->unified = plan.unified;
+    job->c = plan.c;
+    job->W = plan.W;
+    job->D = plan.D;
     auto fail = [&](int s) { job->status = s; return BB_OK; };
     DigitArgs& A = job->dargs;
     A.n = n; A.montgomery = form == BB_FORM_MONTGOMERY;
+    A.scalar_stride = scalar_stride;
     A.base_offset = base_offset;
     A.shard_lo = bases->global_offset; A.shard_n = bases->n; A.global_len = bases->global_len;
     A.c = job->c; A.W = job->W;
@@ -1200,9 +1288,7 @@ int msm_start(bb_ctx* ctx, const bb_bases* bases, size_t base_offset, const uint
     A.table_stride = job->precomp ? (uint32_t)bases->n : 0u;
     A.key_stride = job->unified ? 0u : job->D;
     if (A.win_index >= A.win_count) { set_error("bb_msm: window shard %u of %u", A.win_index, A.win_count); return fail(BB_ERR_ARG); }
-    job->W_local = 0;
-    for (uint32_t w = 0; w < job->W; w++) job->W_local += (w % A.win_count == A.win_index);
-    if (job->W_local == 0) job->W_local = 1;          // degenerate: more shards than windows; slot stays empty
+    job->W_local = plan.W_local;
     int s;
     if (scalars_on_device) A.scalars = (const Fr*)scalars;
     else {
@@ -1280,6 +1366,40 @@ int classify_both_errors(bb_msm_job* job, uint32_t eof_index, int* status) {
 }  // namespace
 
 namespace bb {
+// profile mode: the job's stage times (accumulation, whole job, prover timeline) from its events, then the events go;
+// `cnt` = the job's counter words as copied back (err[4] pairs, err[5] bucket entries)
+void record_profile(bb_msm_job* job, int status, const uint32_t* cnt) {
+    if (job->ev[3]) {
+        float acc_ms = 0, tot_ms = 0;
+        if (status == BB_OK && cudaEventElapsedTime(&acc_ms, job->ev[1], job->ev[2]) == cudaSuccess &&
+            cudaEventElapsedTime(&tot_ms, job->ev[0], job->ev[3]) == cudaSuccess) {
+            bool g2 = job->group == BB_G2;
+            // units: the (base, scalar) pairs this job consumed -- density-selected, non-zero, not Exponent::One,
+            // in this shard (counted by k_msm_digits); entries = non-zero digits of those scalars
+            job->ctx->prof_add(g2 ? "msm_accumulate_g2" : "msm_accumulate_g1", acc_ms, 1, cnt[4]);
+            job->ctx->prof_add(g2 ? "msm_total_g2" : "msm_total_g1", tot_ms, 1, cnt[4]);
+            job->ctx->prof_add(g2 ? "msm_entries_g2" : "msm_entries_g1", acc_ms, 1, cnt[5]);
+            // Fp / Fp2 multiplications of the accumulation stage: halving round r adds entries / 2^(r+1) pairs at 6
+            // each (batch_affine.cuh), the XYZZ stage adds what is left at 10 each -- an upper bound, padding rows and
+            // first entries of a bucket cost nothing
+            uint64_t muls = 0, left = cnt[5];
+            for (uint32_t r = 0; r < job->affine_rounds; r++) { muls += 6 * (left / 2); left -= left / 2; }
+            muls += 10 * left;
+            job->ctx->prof_add(g2 ? "msm_fieldmuls_g2" : "msm_fieldmuls_g1", acc_ms, job->affine_rounds, muls);
+            if (job->tag && job->ctx->epoch_ev) {            // device timeline of the prover: ms since the prove started
+                static const char* const mark[4] = {"start", "acc_start", "acc_end", "end"};
+                for (int i = 0; i < 4; i++) {
+                    float t = 0;
+                    if (cudaEventElapsedTime(&t, job->ctx->epoch_ev, job->ev[i]) == cudaSuccess)
+                        job->ctx->prof_add((std::string("tl.") + job->tag + "." + mark[i]).c_str(), t, 1, 0);
+                }
+            }
+        }
+        for (auto& e : job->ev) if (e) { cudaEventDestroy(e); e = nullptr; }
+        cudaGetLastError();
+    }
+}
+
 // used by prover.cu: wait and return the projective result
 int msm_wait_result(bb_msm_job* job, MsmResult* res) {
     int status = job->status;
@@ -1314,39 +1434,65 @@ int msm_wait_result(bb_msm_job* job, MsmResult* res) {
         }
     }
     res->status = status;
-    if (job->ev[3]) {
-        float acc_ms = 0, tot_ms = 0;
-        if (status == BB_OK && cudaEventElapsedTime(&acc_ms, job->ev[1], job->ev[2]) == cudaSuccess &&
-            cudaEventElapsedTime(&tot_ms, job->ev[0], job->ev[3]) == cudaSuccess) {
-            bool g2 = job->group == BB_G2;
-            // units: the (base, scalar) pairs this job consumed -- density-selected, non-zero, not Exponent::One,
-            // in this shard (counted by k_msm_digits); entries = non-zero digits of those scalars
-            const uint32_t* cnt = (const uint32_t*)((const char*)job->h_out + (size_t)(job->W_out + 1) * (g2 ? sizeof(G2X) : sizeof(G1X)));
-            job->ctx->prof_add(g2 ? "msm_accumulate_g2" : "msm_accumulate_g1", acc_ms, 1, cnt[4]);
-            job->ctx->prof_add(g2 ? "msm_total_g2" : "msm_total_g1", tot_ms, 1, cnt[4]);
-            job->ctx->prof_add(g2 ? "msm_entries_g2" : "msm_entries_g1", acc_ms, 1, cnt[5]);
-            // Fp / Fp2 multiplications of the accumulation stage: halving round r adds entries / 2^(r+1) pairs at 6
-            // each (batch_affine.cuh), the XYZZ stage adds what is left at 10 each -- an upper bound, padding rows and
-            // first entries of a bucket cost nothing
-            uint64_t muls = 0, left = cnt[5];
-            for (uint32_t r = 0; r < job->affine_rounds; r++) { muls += 6 * (left / 2); left -= left / 2; }
-            muls += 10 * left;
-            job->ctx->prof_add(g2 ? "msm_fieldmuls_g2" : "msm_fieldmuls_g1", acc_ms, job->affine_rounds, muls);
-            if (job->tag && job->ctx->epoch_ev) {            // device timeline of the prover: ms since the prove started
-                static const char* const mark[4] = {"start", "acc_start", "acc_end", "end"};
-                for (int i = 0; i < 4; i++) {
-                    float t = 0;
-                    if (cudaEventElapsedTime(&t, job->ctx->epoch_ev, job->ev[i]) == cudaSuccess)
-                        job->ctx->prof_add((std::string("tl.") + job->tag + "." + mark[i]).c_str(), t, 1, 0);
-                }
-            }
-        }
-        for (auto& e : job->ev) if (e) cudaEventDestroy(e);
-        cudaGetLastError();
-    }
+    record_profile(job, status, (const uint32_t*)((const char*)job->h_out + (size_t)(job->W_out + 1) * (job->group == BB_G2 ? sizeof(G2X) : sizeof(G1X))));
     if (job->h_out) job->ctx->pinned_release(job->h_out);
     delete job;
     return status;
+}
+
+// A batched job (msm_start with batch = B): for each proof p, status[p] is what msm_wait_result would report for that
+// vector alone, and points[p] (G1X or G2X) its folded sum where status[p] is BB_OK.  Returns the job-level status (a
+// failure before or during the launch, or of the stream), which then stands for every proof.  Frees the job.
+int msm_wait_batch(bb_msm_job* job, int* status, void* points) {
+    int st = job->status;
+    if (job->ev_done) { cudaEventSynchronize(job->ev_done); cudaEventDestroy(job->ev_done); job->ev_done = nullptr; }
+    cudaError_t e = cudaStreamSynchronize(job->st);
+    if (e != cudaSuccess && st == BB_OK) { set_error("msm stream: %s", cudaGetErrorString(e)); st = BB_ERR_CUDA; }
+    const uint32_t B = job->B;
+    const bool g2 = job->group == BB_G2;
+    const size_t psz = g2 ? sizeof(G2X) : sizeof(G1X);
+    for (uint32_t p = 0; p < B; p++) status[p] = st;
+    if (st == BB_OK && job->h_out) {
+        const uint32_t* err = (const uint32_t*)((const char*)job->h_out + B * psz);
+        const uint32_t* perr = err + 8;
+        const bool eof = err[0] != 0xffffffffu;           // the shape alone decides it: the same for every proof
+        for (uint32_t p = 0; p < B && st == BB_OK; p++) {
+            int s = BB_OK;
+            if (eof && perr[p]) {
+                const DigitArgs saved = job->dargs;
+                job->dargs.scalars += (size_t)p * saved.scalar_stride;
+                int c = g2 ? classify_both_errors<Fp2>(job, err[0], &s) : classify_both_errors<Fp>(job, err[0], &s);
+                job->dargs = saved;
+                if (c != BB_OK) st = c;
+            } else if (eof) {
+                s = BB_ERR_IO_UNEXPECTED_EOF;
+            } else if (perr[p]) {
+                s = BB_ERR_UNEXPECTED_IDENTITY;
+            }
+            status[p] = s;
+        }
+        if (st != BB_OK) for (uint32_t p = 0; p < B; p++) status[p] = st;
+        else std::memcpy(points, job->h_out, B * psz);
+    }
+    record_profile(job, st, job->h_out ? (const uint32_t*)((const char*)job->h_out + B * psz) : nullptr);
+    for (auto& ev : job->ev) if (ev) cudaEventDestroy(ev);      // the events of a job that failed before its last record
+    cudaGetLastError();
+    if (job->h_out) job->ctx->pinned_release(job->h_out);
+    delete job;
+    return st;
+}
+
+// What a batched job of B vectors of n scalars (n_dense of them selected by the density map) over `bases` needs:
+// *slots = its bucket entries (launch_msm refuses 2^32 and more), and an estimate of its device bytes.
+size_t msm_batch_bytes(bb_ctx* ctx, const bb_bases* bases, size_t n, size_t n_dense, uint32_t B, uint64_t* slots) {
+    const bool g2 = bases->group == BB_G2;
+    const MsmPlan p = msm_plan(ctx, bases, true, n, n_dense, B);
+    const uint64_t s = p.slots;
+    *slots = s;
+    const size_t aff = g2 ? sizeof(G2Affine) : sizeof(G1Affine), xyzz = g2 ? sizeof(G2X) : sizeof(G1X), fe = aff / 2;
+    double bytes = 4.0 * s + (double)p.NB * (2.0 * xyzz + 20.0) + (double)(s >> p.R) / 32.0 * (12.0 + xyzz);
+    if (p.R) bytes += (double)s / 2 * (aff + fe) + (double)s / 4 * aff;
+    return (size_t)bytes;
 }
 }  // namespace bb
 

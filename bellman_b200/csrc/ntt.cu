@@ -97,10 +97,16 @@ struct PassArgs {
     int use_post_const;
     int bitrev;
     uint32_t log_n, s0, k, cbits, lowbits;
+    size_t poly_stride;    // grid y = polynomial: src, dst, src_b and src_c of polynomial y start y * poly_stride further
 };
 
 __global__ void __launch_bounds__(256) k_ntt_pass(PassArgs A) {
     extern __shared__ uint32_t sm[];
+    const size_t poff = (size_t)blockIdx.y * A.poly_stride;
+    const Fr* const src = A.src + poff;
+    Fr* const dst = A.dst + poff;
+    const Fr* const src_b = A.src_b ? A.src_b + poff : nullptr;
+    const Fr* const src_c = A.src_b ? A.src_c + poff : nullptr;
     const uint32_t T = 1u << (A.k + A.cbits);
     const uint32_t C = 1u << A.cbits;
     const uint32_t hibits = A.cbits - A.lowbits;
@@ -116,8 +122,8 @@ __global__ void __launch_bounds__(256) k_ntt_pass(PassArgs A) {
     for (uint32_t e = threadIdx.x; e < T; e += blockDim.x) {
         uint32_t p = addr(e);
         uint32_t i = A.bitrev ? (__brev(p) >> (32u - A.log_n)) : p;
-        Fr v = ld_fr(A.src + i);
-        if (A.src_b) v = v * ld_fr(A.src_b + i) - ld_fr(A.src_c + i);
+        Fr v = ld_fr(src + i);
+        if (src_b) v = v * ld_fr(src_b + i) - ld_fr(src_c + i);
         if (A.pre) v = v * ld_fr(A.pre + i);
 #pragma unroll
         for (int w = 0; w < 8; w++) sm[w * T + e] = v.l[w];
@@ -150,7 +156,7 @@ __global__ void __launch_bounds__(256) k_ntt_pass(PassArgs A) {
         for (int w = 0; w < 8; w++) v.l[w] = sm[w * T + e];
         if (A.post) v = v * ld_fr(A.post + p);
         if (A.use_post_const) v = v * A.post_const;
-        st_fr(A.dst + p, v);
+        st_fr(dst + p, v);
     }
 }
 
@@ -166,6 +172,11 @@ static __device__ __noinline__ Fr fr_mul_outlined(Fr a, Fr b) { return a * b; }
 // one stores straight from them.  Twiddles: 7 per thread and window (1 + 2 + 4), read-only path.
 __global__ void __launch_bounds__(256) k_ntt_pass8(PassArgs A) {
     extern __shared__ uint32_t sm[];
+    const size_t poff = (size_t)blockIdx.y * A.poly_stride;
+    const Fr* const src = A.src + poff;
+    Fr* const dst = A.dst + poff;
+    const Fr* const src_b = A.src_b ? A.src_b + poff : nullptr;
+    const Fr* const src_c = A.src_b ? A.src_c + poff : nullptr;
     const uint32_t T = 1u << (A.k + A.cbits);
     const uint32_t C = 1u << A.cbits;
     const uint32_t hibits = A.cbits - A.lowbits;
@@ -192,8 +203,8 @@ __global__ void __launch_bounds__(256) k_ntt_pass8(PassArgs A) {
             for (uint32_t u = 0; u < 8; u++) {
                 uint32_t p = addr(e0 | (u << sh));
                 uint32_t i = A.bitrev ? (__brev(p) >> (32u - A.log_n)) : p;
-                Fr v = ld_fr(A.src + i);
-                if (A.src_b) v = v * ld_fr(A.src_b + i) - ld_fr(A.src_c + i);
+                Fr v = ld_fr(src + i);
+                if (src_b) v = v * ld_fr(src_b + i) - ld_fr(src_c + i);
                 if (A.pre) v = v * ld_fr(A.pre + i);
                 x[u] = v;
             }
@@ -241,7 +252,7 @@ __global__ void __launch_bounds__(256) k_ntt_pass8(PassArgs A) {
                 Fr v = x[u];
                 if (A.post) v = v * ld_fr(A.post + p);
                 if (A.use_post_const) v = v * A.post_const;
-                st_fr(A.dst + p, v);
+                st_fr(dst + p, v);
             }
         }
     }
@@ -319,16 +330,18 @@ struct Fusion {
     Fr post_const_v;
 };
 
-// One transform: data (natural order) -> data, scratch tmp of the same size.
+// One transform: data (natural order) -> data, scratch tmp of the same size.  polys > 1: the same transform of `polys`
+// polynomials at src, data, tmp (and the fused src_b, src_c) + j * stride, j < polys, in the same launches (grid y).
 static int run_passes(bb_ctx* ctx, cudaStream_t st, const Fr* src, Fr* data, Fr* tmp, uint32_t log_n,
-                      const Fr* tw, const Fusion& fu) {
+                      const Fr* tw, const Fusion& fu, uint32_t polys = 1, size_t stride = 0) {
     if (log_n == 0) {
         // single point: only the fused multiplications apply
         PassArgs A{};
         A.src = src; A.dst = data; A.src_b = fu.src_b; A.src_c = fu.src_c; A.tw = tw; A.pre = fu.pre; A.post = fu.post;
         A.use_post_const = fu.post_const; A.post_const = fu.post_const_v; A.bitrev = 0;
         A.log_n = 0; A.s0 = 0; A.k = 0; A.cbits = 0; A.lowbits = 0;
-        k_ntt_pass<<<1, 32, 32, st>>>(A);
+        A.poly_stride = stride;
+        k_ntt_pass<<<dim3(1, polys), 32, 32, st>>>(A);
         ctx->count_launch();
         BB_CUDA(cudaGetLastError());
         return BB_OK;
@@ -357,9 +370,10 @@ static int run_passes(bb_ctx* ctx, cudaStream_t st, const Fr* src, Fr* data, Fr*
         A.bitrev = first;
         A.log_n = log_n; A.s0 = s0; A.k = k; A.cbits = cbits;
         A.lowbits = s0 < cbits ? s0 : cbits;
+        A.poly_stride = stride;
         size_t smem = ((size_t)32) << (k + cbits);
         if (smem > 48 * 1024) BB_CUDA(cudaFuncSetAttribute(k_ntt_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        unsigned grid = 1u << (log_n - k - cbits);
+        const dim3 grid(1u << (log_n - k - cbits), polys);
         unsigned threads = (1u << (k + cbits)) / 2 < 256 ? ((1u << (k + cbits)) / 2 < 32 ? 32 : (1u << (k + cbits)) / 2) : 256;
         // register radix-8 windows: 8 elements per thread, three row bits at a time (k >= 3), at least one warp per tile
         const bool r8 = ctx->opt_ntt_radix8 && k >= 3 && (k + cbits) >= 8 && (k + cbits) <= 11;
@@ -371,7 +385,10 @@ static int run_passes(bb_ctx* ctx, cudaStream_t st, const Fr* src, Fr* data, Fr*
         BB_CUDA(cudaGetLastError());
         s0 += k;
     }
-    if (npass == 1) BB_CUDA(cudaMemcpyAsync(data, tmp, sizeof(Fr) << log_n, cudaMemcpyDeviceToDevice, st));
+    if (npass == 1) {
+        if (polys == 1) BB_CUDA(cudaMemcpyAsync(data, tmp, sizeof(Fr) << log_n, cudaMemcpyDeviceToDevice, st));
+        else BB_CUDA(cudaMemcpy2DAsync(data, stride * sizeof(Fr), tmp, stride * sizeof(Fr), sizeof(Fr) << log_n, polys, cudaMemcpyDeviceToDevice, st));
+    }
     return BB_OK;
 }
 
@@ -424,6 +441,28 @@ int h_poly_device(bb_ctx* ctx, cudaStream_t st, Fr* d_a, Fr* d_b, Fr* d_c, Fr* d
     Fusion fin;                         // mul_assign, sub_assign, divide_by_z_on_coset, icoset_fft (:232-237)
     fin.src_b = d_b; fin.src_c = d_c; fin.post = gz;
     return run_passes(ctx, st, d_a, d_a, d_tmp, log_m, tw_i, fin);
+}
+
+// h_poly_device for B proofs in the same launches: d_abc holds a_0 .. a_{B-1}, b_0 .. b_{B-1}, c_0 .. c_{B-1}, m = 2^log_m
+// elements each (zero padded); d_tmp the same 3 B m.  The 3 B inverse and forward transforms run as one pass sequence
+// each, the final transform as one over the B products: 3 pass sequences per sub-batch.  h_j is left in a_j.
+int h_poly_batch_device(bb_ctx* ctx, cudaStream_t st, Fr* d_abc, Fr* d_tmp, uint32_t log_m, uint32_t B) {
+    if (log_m >= (uint32_t)bbc::FR_S) { set_error("2^%u-point domain: PolynomialDegreeTooLarge", log_m); return BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE; }
+    NttTables* t = nullptr;
+    const Fr *tw_f = nullptr, *tw_i = nullptr, *gm = nullptr, *gz = nullptr;
+    BB_TRY(get_table(ctx, st, log_m, T_TW_FWD, &t, &tw_f));
+    BB_TRY(get_table(ctx, st, log_m, T_TW_INV, &t, &tw_i));
+    BB_TRY(get_table(ctx, st, log_m, T_POW_G_MINV, &t, &gm));
+    BB_TRY(get_table(ctx, st, log_m, T_POW_GINV_MINV_ZINV, &t, &gz));
+    const size_t m = (size_t)1 << log_m;
+    Fusion inv;                         // ifft with the coset shift fused (:225-230), all 3 B polynomials
+    inv.post = gm;
+    BB_TRY(run_passes(ctx, st, d_abc, d_abc, d_tmp, log_m, tw_i, inv, 3 * B, m));
+    Fusion fwd;                         // the fft half of coset_fft
+    BB_TRY(run_passes(ctx, st, d_abc, d_abc, d_tmp, log_m, tw_f, fwd, 3 * B, m));
+    Fusion fin;                         // a*b - c, divide_by_z_on_coset, icoset_fft (:232-237), B polynomials
+    fin.src_b = d_abc + (size_t)B * m; fin.src_c = d_abc + 2 * (size_t)B * m; fin.post = gz;
+    return run_passes(ctx, st, d_abc, d_abc, d_tmp, log_m, tw_i, fin, B, m);
 }
 
 // The two halves of h_poly_device for the multi-GPU split by polynomial: the coset evaluations of one

@@ -1,6 +1,10 @@
 // bellman_b200: the device side of groth16::create_proof after synthesis
 // (bellman/groth16/src/prover.rs:217-360): CRS residency, the H pipeline, the eight
 // multiexps in flight, and the host finalisation.
+#include <sched.h>
+
+#include <algorithm>
+#include <atomic>
 #include <chrono>
 #include <functional>
 #include <memory>
@@ -201,19 +205,32 @@ void bb_crs_destroy(bb_crs* crs) {
 
 namespace {
 
-// x_i / zz_i, y_i / zzz_i for a handful of points with ONE field inversion (Montgomery's trick)
+// x_i / zz_i, y_i / zzz_i for n points with ONE field inversion (Montgomery's trick)
 template <class F>
-void batch_to_affine(const XYZZ<F>* in, int n, Affine<F>* out) {
-    F pre[8];
+void batch_to_affine(const XYZZ<F>* in, size_t n, Affine<F>* out) {
+    std::vector<F> pre(n);
     F acc = FieldOps<F>::one();
-    for (int i = 0; i < n; i++) { pre[i] = acc; if (!in[i].is_identity()) acc = acc * in[i].ZZZ; }
+    for (size_t i = 0; i < n; i++) { pre[i] = acc; if (!in[i].is_identity()) acc = acc * in[i].ZZZ; }
     F inv = FieldOps<F>::inv(acc);
-    for (int i = n - 1; i >= 0; i--) {
+    for (size_t i = n; i-- > 0;) {
         if (in[i].is_identity()) { out[i] = Affine<F>::identity(); continue; }
         F zi3 = inv * pre[i];
         inv = inv * in[i].ZZZ;
         F zi2 = (zi3 * in[i].ZZ).sqr();
         out[i] = {in[i].X * zi2, in[i].Y * zi3};
+    }
+}
+
+// The message bb_groth16_prove reports with status s for this key (NULL for the back-end statuses, whose text varies)
+const char* prove_status_message(const bb_crs* crs, int s) {
+    switch (s) {
+        case BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE: return "PolynomialDegreeTooLarge";
+        case BB_ERR_UNEXPECTED_IDENTITY:
+            return crs->delta_g1.is_identity() || crs->delta_g2.is_identity() ? "delta is the identity: subversion-CRS attack"
+                                                                              : "encountered an identity element in the CRS";
+        case BB_ERR_IO_UNEXPECTED_EOF: return "expected more bases from source";
+        case BB_ERR_DENSITY_MISMATCH: return "density map length differs from the number of exponents";
+        default: return nullptr;
     }
 }
 
@@ -396,10 +413,7 @@ int prove_end_impl(bb_prove* Praw, const void* const* evals, uint8_t* partials, 
         if (s == BB_OK && delta_is_identity(crs)) s = BB_ERR_UNEXPECTED_IDENTITY;
         for (int idx = 0; idx < 8 && s == BB_OK; idx++) s = slot_status[ref_wait_order[idx]];
         // the message of the error that is reported (another job may have failed later)
-        if (s == BB_ERR_IO_UNEXPECTED_EOF) set_error("expected more bases from source");
-        else if (s == BB_ERR_UNEXPECTED_IDENTITY && !crs->delta_g1.is_identity() && !crs->delta_g2.is_identity())
-            set_error("encountered an identity element in the CRS");
-        else if (s == BB_ERR_DENSITY_MISMATCH) set_error("density map length differs from the number of exponents");
+        if (const char* msg = prove_status_message(crs, s)) set_error("%s", msg);
     }
     if (s == BB_OK) {
         G1Affine a1[6];
@@ -473,7 +487,301 @@ int finalize_impl(const bb_crs* crs, const uint8_t* partials, size_t count, cons
     return BB_OK;
 }
 
+
+// ---- many witnesses of one circuit against one key (bb_groth16_prove_batch) --------------------------------------------
+// A sub-batch of B items is one H pipeline per item on the main stream and EIGHT MSM jobs, each over the B scalar vectors of
+// its slot (msm_start with batch = B): the launches per sub-batch are those of one proof plus B - 1 H pipelines, and the
+// window folds run on the device.  The host work -- the scalar multiplications by r, s, rs -- is the single-proof code,
+// run for the items side by side.
+
+// fn(i) for i < n on a pool of host threads, one per CPU this process may run on
+void parallel_for(size_t n, const std::function<void(size_t)>& fn) {
+    if (!n) return;
+    size_t cpus = 1;
+    cpu_set_t set;
+    if (sched_getaffinity(0, sizeof set, &set) == 0) cpus = (size_t)CPU_COUNT(&set);
+    const size_t k = std::max<size_t>(1, std::min(cpus, n));
+    std::atomic<size_t> next{0};
+    auto body = [&] { for (size_t i; (i = next.fetch_add(1)) < n;) fn(i); };
+    std::vector<std::thread> pool;
+    for (size_t j = 1; j < k; j++) pool.emplace_back(body);
+    body();
+    for (auto& th : pool) th.join();
+}
+
+size_t density_count(const uint64_t* bits, size_t n) {
+    if (!bits) return n;
+    size_t c = 0;
+    for (size_t j = 0; j < (n + 63) / 64; j++) {
+        uint64_t wv = bits[j];
+        if (j == (n + 63) / 64 - 1 && (n & 63)) wv &= (1ull << (n & 63)) - 1ull;
+        c += (size_t)__builtin_popcountll(wv);
+    }
+    return c;
+}
+
+bool same_density(const uint64_t* a, const uint64_t* b, size_t bits) {
+    if (!a || !b) return a == b;
+    return std::memcmp(a, b, (bits + 63) / 64 * 8) == 0;
+}
+
+size_t domain_size(size_t n, uint32_t* log_m) {
+    size_t m = 1;
+    *log_m = 0;
+    while (m < n && *log_m < 63) { m *= 2; *log_m += 1; }
+    return m;
+}
+
+// One sub-batch in flight: the buffers of its B items and its eight jobs.  Every exit drains the jobs and the streams.
+struct BatchRun {
+    bb_ctx* ctx = nullptr;
+    uint32_t B = 0;
+    DevBuf d_in, d_aux, d_abc, d_tmp;
+    cudaStream_t up = nullptr;
+    cudaEvent_t ev_up = nullptr, ev_h = nullptr;
+    bb_msm_job* jobs[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    ~BatchRun() {
+        std::vector<int> st(B ? B : 1);
+        std::vector<G2X> pts(B ? B : 1);
+        for (auto& j : jobs) if (j) { msm_wait_batch(j, st.data(), pts.data()); j = nullptr; }
+        if (ctx) cudaStreamSynchronize(ctx->main_stream);
+        if (up) cudaStreamSynchronize(up);
+        if (ev_up) cudaEventDestroy(ev_up);
+        if (ev_h) cudaEventDestroy(ev_h);
+    }
+};
+
+// The eight jobs of a proof (bases, base offset, density, scalars, scalars the density selects) in slot order
+struct SlotShape { const bb_bases* bases; size_t off; const uint64_t* dens; size_t n; size_t n_dense; };
+void slot_shapes(const bb_crs* crs, const bb_witness* w, size_t m, SlotShape out[8]) {
+    const size_t b_in_total = density_count(w->b_input_density, w->n_inputs);
+    out[0] = {crs->h, 0, nullptr, m - 1, m - 1};
+    out[1] = {crs->l, 0, nullptr, w->n_aux, w->n_aux};
+    out[2] = {crs->a, 0, nullptr, w->n_inputs, w->n_inputs};
+    out[3] = {crs->a, w->n_inputs, w->a_aux_density, w->n_aux, density_count(w->a_aux_density, w->n_aux)};
+    out[4] = {crs->b_g1, 0, w->b_input_density, w->n_inputs, b_in_total};
+    out[5] = {crs->b_g1, b_in_total, w->b_aux_density, w->n_aux, density_count(w->b_aux_density, w->n_aux)};
+    out[6] = {crs->b_g2, 0, w->b_input_density, w->n_inputs, b_in_total};
+    out[7] = {crs->b_g2, b_in_total, w->b_aux_density, w->n_aux, density_count(w->b_aux_density, w->n_aux)};
+}
+
+// Proofs per sub-batch: prove_batch_max if set, and at most what one job's 2^32 bucket entries, its result staging block
+// and the device memory (free plus the context's cached blocks, against an estimate per proof) hold
+size_t batch_limit(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t count) {
+    uint32_t log_m;
+    const size_t m = domain_size(w->n_constraints, &log_m);
+    SlotShape js[8];
+    slot_shapes(crs, w, m, js);
+    size_t k = count;
+    if (ctx->opt_prove_batch_max > 0) k = std::min(k, (size_t)ctx->opt_prove_batch_max);
+    k = std::min(k, (bb_ctx::PINNED_BLOCK - 32) / (sizeof(G2X) + 4));
+    size_t free_b = 0, total_b = 0;
+#if defined(__CUDACC__)
+    if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); free_b = 0; }
+#else
+    free_b = (size_t)1 << 40;                          // the sources compiled for host threads (tests/native): no device to ask
+#endif
+    {
+        std::lock_guard<std::mutex> g(ctx->mu);
+        for (auto& kv : ctx->free_blocks) free_b += kv.first;
+    }
+    const double budget = 0.85 * (double)free_b;
+    auto fits = [&](size_t b) {
+        double bytes = (double)b * (6 * m + w->n_inputs + w->n_aux) * 32.0;        // a, b, c and their scratch; the witnesses
+        for (auto& j : js) {
+            if (!j.bases) continue;
+            uint64_t slots = 0;
+            bytes += (double)msm_batch_bytes(ctx, j.bases, j.n, j.n_dense, (uint32_t)b, &slots);
+            if (slots >= (1ull << 32)) return false;
+        }
+        return bytes <= budget;
+    };
+    while (k > 1 && !fits(k)) k -= std::max<size_t>(1, k / 8);
+    return std::max<size_t>(1, k);
+}
+
+// Items 0 .. B - 1 of w: queue, wait, finalise.  Returns a failure of the sub-batch as a whole (it then stands for every
+// item); otherwise status[] holds each item's bb_groth16_prove status.
+int prove_sub_batch(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, uint32_t B, const uint8_t* r_bytes, const uint8_t* s_bytes,
+                    uint8_t* proofs, int* status, double* host_tail_ms, const BatchAbcFill* fill) {
+    const bb_witness& w0 = w[0];
+    const size_t n = w0.n_constraints, ni = w0.n_inputs, na = w0.n_aux;
+    uint32_t log_m;
+    const size_t m = domain_size(n, &log_m);
+    const cudaMemcpyKind kind = w0.on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    cudaStream_t st = ctx->main_stream;
+    BatchRun run;
+    run.ctx = ctx; run.B = B;
+    BB_TRY(run.d_abc.alloc(ctx, (size_t)3 * B * m * 32)); BB_TRY(run.d_tmp.alloc(ctx, (size_t)3 * B * m * 32));
+    BB_TRY(run.d_in.alloc(ctx, (size_t)B * ni * 32)); BB_TRY(run.d_aux.alloc(ctx, (size_t)B * na * 32));
+    run.up = ctx->pick_stream();
+    BB_CUDA(cudaEventCreateWithFlags(&run.ev_up, cudaEventDisableTiming));
+    BB_CUDA(cudaEventCreateWithFlags(&run.ev_h, cudaEventDisableTiming));
+    for (uint32_t i = 0; i < B; i++) {
+        if (ni) BB_CUDA(cudaMemcpyAsync((char*)run.d_in.p + (size_t)i * ni * 32, w[i].input_assignment, ni * 32, kind, run.up));
+        if (na) BB_CUDA(cudaMemcpyAsync((char*)run.d_aux.p + (size_t)i * na * 32, w[i].aux_assignment, na * 32, kind, run.up));
+    }
+    if (!w0.on_device) ctx->h2d_bytes += (size_t)B * (ni + na) * 32;
+    BB_CUDA(cudaEventRecord(run.ev_up, run.up));
+    // the H pipeline (prover.rs:221-240) of the whole sub-batch on the main stream: rows a_0 .. a_{B-1}, b_0 .., c_0 .. of
+    // m Fr, zero padded; item i's h coefficients are left in a_i
+    {
+        NvtxRange range("bb: batch H pipeline");
+        Fr* abc = run.d_abc.as<Fr>();
+        if (fill) {                                      // a, b, c evaluated on the device from the uploaded witnesses
+            BB_CUDA(cudaStreamWaitEvent(st, run.ev_up, 0));
+            BB_TRY((*fill)(st, B, abc, m, run.d_in.as<Fr>(), run.d_aux.as<Fr>()));
+        } else {
+            for (uint32_t i = 0; i < B; i++) {
+                const void* srcs[3] = {w[i].a, w[i].b, w[i].c};
+                for (uint32_t k = 0; k < 3 && n; k++)
+                    BB_CUDA(cudaMemcpyAsync(abc + ((size_t)k * B + i) * m, srcs[k], n * 32, kind, st));
+            }
+            if (!w0.on_device) ctx->h2d_bytes += (size_t)B * 3 * n * 32;
+        }
+        if (m > n) BB_CUDA(cudaMemset2DAsync(abc + n, m * 32, 0, (m - n) * 32, (size_t)3 * B, st));   // coeffs.resize(m, zero), domain.rs:69
+        BB_TRY(h_poly_batch_device(ctx, st, abc, run.d_tmp.as<Fr>(), log_m, B));
+        BB_CUDA(cudaEventRecord(run.ev_h, st));
+    }
+    SlotShape js[8];
+    slot_shapes(crs, &w0, m, js);
+    const void* src[8] = {run.d_abc.p, run.d_aux.p, run.d_in.p, run.d_aux.p, run.d_in.p, run.d_aux.p, run.d_in.p, run.d_aux.p};
+    const size_t stride[8] = {m, na, ni, na, ni, na, ni, na};
+    int s = BB_OK;
+    for (int slot : {0, 7, 1, 2, 3, 4, 5, 6}) {           // prove_begin's order: h, the G2 job, then the rest
+        const SlotShape& j = js[slot];
+        if (s == BB_OK)
+            s = msm_start(ctx, j.bases, j.off, j.dens, j.dens ? j.n : 0, src[slot], true, j.n, BB_FORM_MONTGOMERY, slot == 0 ? run.ev_h : run.ev_up,
+                          &run.jobs[slot], job_tag[slot], slot == 0 ? 1 : slot == 7 ? 2 : 0, B, stride[slot]);
+    }
+    if (s != BB_OK) return s;
+    // while the device works: the MSM-independent terms of every item
+    std::vector<ProofStatic> stat(B);
+    std::vector<Fr> rr(B), ss(B);
+    for (uint32_t i = 0; i < B; i++) { std::memcpy(rr[i].l, r_bytes + 32 * i, 32); std::memcpy(ss[i].l, s_bytes + 32 * i, 32); }
+    const bool bad_delta = crs->delta_g1.is_identity() || crs->delta_g2.is_identity();
+    if (!bad_delta) parallel_for(B, [&](size_t i) { finalize_static(crs, rr[i], ss[i], &stat[i]); });
+    std::vector<int> slot_status[8];
+    std::vector<G1X> sums1[6];
+    std::vector<G2X> sums2[2];
+    int job_status[8] = {BB_OK, BB_OK, BB_OK, BB_OK, BB_OK, BB_OK, BB_OK, BB_OK};
+    {
+        std::thread waiters[8];
+        for (int k = 0; k < 8; k++) {
+            slot_status[k].assign(B, BB_OK);
+            if (k < 6) sums1[k].assign(B, G1X::identity()); else sums2[k - 6].assign(B, G2X::identity());
+            bb_msm_job* job = run.jobs[k];
+            run.jobs[k] = nullptr;
+            if (!job) continue;
+            waiters[k] = std::thread([&, k, job] {
+                cudaSetDevice(ctx->device);
+                void* pts = k < 6 ? (void*)sums1[k].data() : (void*)sums2[k - 6].data();
+                job_status[k] = msm_wait_batch(job, slot_status[k].data(), pts);
+            });
+        }
+        for (auto& th : waiters) if (th.joinable()) th.join();
+    }
+    const auto t_waited = std::chrono::steady_clock::now();
+    // the density assert is a per-item status; anything else a job failed with is the sub-batch's
+    for (int k = 0; k < 8; k++) if (job_status[k] != BB_OK && job_status[k] != BB_ERR_DENSITY_MISMATCH) return job_status[k];
+    // each item's status as prove_end_impl decides it for a single proof
+    static const int ref_wait_order[8] = {2, 3, 4, 5, 6, 7, 0, 1};
+    std::vector<uint32_t> ok;
+    for (uint32_t i = 0; i < B; i++) {
+        int si = BB_OK;
+        for (int k = 0; k < 8 && si == BB_OK; k++) if (slot_status[k][i] == BB_ERR_DENSITY_MISMATCH) si = BB_ERR_DENSITY_MISMATCH;
+        if (si == BB_OK && bad_delta) si = BB_ERR_UNEXPECTED_IDENTITY;
+        for (int idx = 0; idx < 8 && si == BB_OK; idx++) si = slot_status[ref_wait_order[idx]][i];
+        status[i] = si;
+        if (si == BB_OK) ok.push_back(i);
+    }
+    // to affine: one inversion for all G1 points of the sub-batch and one for all G2 points
+    const size_t nk = ok.size();
+    std::vector<G1X> p1(6 * nk);
+    std::vector<G2X> p2(2 * nk);
+    for (size_t q = 0; q < nk; q++) {
+        for (int k = 0; k < 6; k++) p1[6 * q + k] = sums1[k][ok[q]];
+        for (int k = 0; k < 2; k++) p2[2 * q + k] = sums2[k][ok[q]];
+    }
+    std::vector<G1Affine> a1(6 * nk);
+    std::vector<G2Affine> a2(2 * nk);
+    batch_to_affine<Fp>(p1.data(), p1.size(), a1.data());
+    batch_to_affine<Fp2>(p2.data(), p2.size(), a2.data());
+    parallel_for(nk, [&](size_t q) {
+        const uint32_t i = ok[q];
+        uint8_t partials[BB_PARTIALS_BYTES];
+        std::memcpy(partials, &a1[6 * q], 6 * 96);
+        std::memcpy(partials + 576, &a2[2 * q], 2 * 192);
+        finalize_impl(crs, partials, 1, rr[i], ss[i], stat[i], proofs + (size_t)i * BB_PROOF_BYTES);
+    });
+    *host_tail_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_waited).count();
+    return BB_OK;
+}
+
 }  // namespace
+
+namespace bb {
+
+int prove_batch_check(const char* fn, const bb_ctx* ctx, const bb_crs* crs, size_t count, const void* r, const void* s, const void* proofs,
+                      const int* status) {
+    if (!ctx || !crs || crs->ctx != ctx) { set_error("%s: null argument or a key of another context", fn); return BB_ERR_ARG; }
+    if (crs->shard_count != 1) { set_error("%s needs an unsharded CRS", fn); return BB_ERR_ARG; }
+    if (count && (!r || !s || !proofs || !status)) { set_error("%s: null argument", fn); return BB_ERR_ARG; }
+    return BB_OK;
+}
+
+int prove_batch_impl(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t count, const uint8_t* r, const uint8_t* s,
+                     uint8_t* proofs, int* status, const BatchAbcFill* fill) {
+    BB_TRY(prove_batch_check("bb_groth16_prove_batch", ctx, crs, count, r, s, proofs, status));
+    if (!count) return BB_OK;
+    if (!w) { set_error("bb_groth16_prove_batch: null argument"); return BB_ERR_ARG; }
+    const bb_witness& w0 = w[0];
+    for (size_t i = 0; i < count; i++) {
+        const bb_witness& wi = w[i];
+        if (wi.n_constraints != w0.n_constraints || wi.n_inputs != w0.n_inputs || wi.n_aux != w0.n_aux || (wi.on_device != 0) != (w0.on_device != 0) ||
+            !same_density(wi.a_aux_density, w0.a_aux_density, w0.n_aux) || !same_density(wi.b_input_density, w0.b_input_density, w0.n_inputs) ||
+            !same_density(wi.b_aux_density, w0.b_aux_density, w0.n_aux)) {
+            set_error("bb_groth16_prove_batch: item %zu differs from item 0 in its shape or its densities", i);
+            return BB_ERR_ARG;
+        }
+        if ((wi.n_constraints && !fill && (!wi.a || !wi.b || !wi.c)) || (wi.n_inputs && !wi.input_assignment) || (wi.n_aux && !wi.aux_assignment) ||
+            (wi.n_inputs && !wi.b_input_density) || (wi.n_aux && (!wi.a_aux_density || !wi.b_aux_density))) {
+            set_error("bb_groth16_prove_batch: item %zu has a null array", i);
+            return BB_ERR_ARG;
+        }
+    }
+    std::memset(proofs, 0, count * BB_PROOF_BYTES);
+    uint32_t log_m;
+    domain_size(w0.n_constraints, &log_m);
+    if (log_m >= (uint32_t)bbc::FR_S) {                   // from_coeffs, domain.rs:49-60: every item alike
+        set_error("%s", prove_status_message(crs, BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE));
+        for (size_t i = 0; i < count; i++) status[i] = BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE;
+        return BB_OK;
+    }
+    BB_CUDA(cudaSetDevice(ctx->device));
+    NvtxRange range("bb: prove_batch");
+    if (ctx->opt_profile) {                           // origin of the jobs' device timeline (bb_profile_read "tl.<job>.<mark>")
+        if (!ctx->epoch_ev) BB_CUDA(cudaEventCreate(&ctx->epoch_ev));
+        BB_CUDA(cudaEventRecord(ctx->epoch_ev, ctx->main_stream));
+    }
+    const size_t k = batch_limit(ctx, crs, &w0, count);
+    double tail = 0;
+    size_t subs = 0;
+    for (size_t lo = 0; lo < count; lo += k, subs++) {
+        const uint32_t B = (uint32_t)std::min(k, count - lo);
+        const int rc = prove_sub_batch(ctx, crs, w + lo, B, r + 32 * lo, s + 32 * lo, proofs + lo * BB_PROOF_BYTES, status + lo, &tail, fill);
+        for (uint32_t i = 0; i < B; i++) {
+            if (rc != BB_OK) status[lo + i] = rc;          // a failure of the sub-batch as a whole: none of its items has a proof
+            if (status[lo + i] != BB_OK) std::memset(proofs + (lo + i) * BB_PROOF_BYTES, 0, BB_PROOF_BYTES);
+        }
+    }
+    if (ctx->opt_profile) {
+        ctx->prof_add("prove_batch.host_tail", tail, subs, count);      // host ms from the last MSM result to the proof bytes
+        ctx->prof_add("prove_batch.sub_batches", 0, subs, count);
+    }
+    return BB_OK;
+}
+}  // namespace bb
 
 extern "C" {
 
@@ -706,6 +1014,13 @@ int bb_groth16_prove(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, const 
         ctx->prof_add("host.proof_done", since(), 1, 0);
     }
     return rc;
+}
+
+const char* bb_groth16_prove_message(const bb_crs* crs, int status) { return crs ? prove_status_message(crs, status) : nullptr; }
+
+int bb_groth16_prove_batch(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t count, const uint8_t* r, const uint8_t* s,
+                           uint8_t* proofs, int* status) {
+    return prove_batch_impl(ctx, crs, w, count, r, s, proofs, status);
 }
 
 }  // extern "C"

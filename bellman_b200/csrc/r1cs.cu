@@ -14,6 +14,7 @@
 //   taken before);
 //   the row ids binned by length: <= 32 terms one thread per row, 33..2048 one warp per row,
 //   more one CTA of 256 threads per row.
+#include <algorithm>
 #include <memory>
 #include <vector>
 
@@ -322,6 +323,34 @@ int bb_groth16_prove_r1cs(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* R, cons
     const int rc = bb_groth16_prove(ctx, crs, &w, r, s, proof);
     if (cudaStreamSynchronize(st) == cudaSuccess) tm.report(R->nnz[0] + R->nnz[1] + R->nnz[2]);
     return rc;
+}
+
+// bb_groth16_prove_batch with the evaluation as its fill: each sub-batch uploads its witnesses once and evaluates every
+// item's a, b, c straight into the rows its H pipeline transforms
+int bb_groth16_prove_r1cs_batch(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* R, const void* inputs, size_t n_inputs, const void* aux,
+                                size_t n_aux, size_t count, int on_device, const uint8_t* r, const uint8_t* s, uint8_t* proofs, int* status) {
+    if (!R) { set_error("bb_groth16_prove_r1cs_batch: null argument"); return BB_ERR_ARG; }
+    if (!count) return prove_batch_impl(ctx, crs, nullptr, 0, r, s, proofs, status);
+    BB_TRY(check_witness("bb_groth16_prove_r1cs_batch", ctx, R, inputs, n_inputs, aux, n_aux, on_device, true));
+    const size_t n = R->n;
+    std::vector<bb_witness> ws(count);
+    for (size_t i = 0; i < count; i++) {
+        bb_witness& w = ws[i];
+        w.n_constraints = n; w.n_inputs = n_inputs; w.n_aux = n_aux;
+        w.input_assignment = (const char*)inputs + i * n_inputs * 32;
+        w.aux_assignment = n_aux ? (const char*)aux + i * n_aux * 32 : nullptr;
+        w.a_aux_density = R->a_aux_density.data();
+        w.b_input_density = R->b_input_density.data();
+        w.b_aux_density = R->b_aux_density.data();
+        w.on_device = on_device;
+    }
+    const BatchAbcFill fill = [&](cudaStream_t st, uint32_t B, Fr* abc, size_t m, const Fr* d_in, const Fr* d_aux) -> int {
+        for (uint32_t i = 0; i < B; i++)
+            BB_TRY(r1cs_eval_queue(ctx, st, R, d_in + (size_t)i * n_inputs, d_aux + (size_t)i * n_aux, abc + (size_t)i * m,
+                                   abc + ((size_t)B + i) * m, abc + (2 * (size_t)B + i) * m));
+        return BB_OK;
+    };
+    return prove_batch_impl(ctx, crs, ws.data(), count, r, s, proofs, status, &fill);
 }
 
 }  // extern "C"

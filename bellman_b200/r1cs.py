@@ -169,3 +169,41 @@ def create_random_proof_r1cs(r1cs, params, input_assignment, aux_assignment, rng
     draw = rng.randrange if rng is not None else secrets.randbelow
     return create_proof_r1cs(r1cs, params, input_assignment, aux_assignment, draw(FR_MODULUS), draw(FR_MODULUS), device_ptrs)
 
+
+
+def create_proof_r1cs_batch(r1cs, params, inputs, aux, rs, ss, device_ptrs=None):
+    """bb_groth16_prove_r1cs_batch: create_proof_r1cs for len(rs) witnesses of this constraint system in one call.
+    inputs / aux: one witness per item (count x n_inputs and count x n_aux Fr), or device_ptrs = dict inputs, aux -> device
+    addresses of those two row-major arrays.  Returns one entry per item: its 192 bytes, or the exception
+    create_proof_r1cs would raise for it alone (an instance, not raised)."""
+    from . import _batch_result, _scalars_bytes
+    count = len(rs)
+    if len(ss) != count:
+        raise ValueError("create_proof_r1cs_batch: one r and one s per item")
+    if device_ptrs is not None:
+        src = (C.c_void_p(_addr(device_ptrs["inputs"])), C.c_size_t(r1cs.n_inputs), C.c_void_p(_addr(device_ptrs["aux"])),
+               C.c_size_t(r1cs.n_aux), C.c_size_t(count), C.c_int(1))
+        keep = ()
+    else:
+        inp = np.ascontiguousarray(np.asarray(inputs, dtype=np.uint64).reshape(count, -1, 4))
+        ax = np.ascontiguousarray(np.asarray(aux, dtype=np.uint64).reshape(count, -1, 4))
+        src = (_ptr(inp), C.c_size_t(inp.shape[1]), _ptr(ax), C.c_size_t(ax.shape[1]), C.c_size_t(count), C.c_int(0))
+        keep = (inp, ax)
+    proofs = (C.c_uint8 * (192 * max(count, 1)))()
+    status = (C.c_int * max(count, 1))()
+    rc = load_library().bb_groth16_prove_r1cs_batch(params.worker._h, params._h, r1cs._h, *src, _scalars_bytes(rs), _scalars_bytes(ss),
+                                                    proofs, status)
+    del keep
+    return _batch_result(params, rc, proofs, list(status)[:count])
+
+
+def create_random_proof_r1cs_batch(r1cs, params, inputs, aux, count=None, rng=None, device_ptrs=None):
+    """create_random_proof_r1cs for each witness: fresh (r, s) per item, then create_proof_r1cs_batch"""
+    import secrets
+    draw = rng.randrange if rng is not None else secrets.randbelow
+    count = len(inputs) if count is None else count
+    rs, ss = [], []
+    for _ in range(count):
+        rs.append(draw(FR_MODULUS))
+        ss.append(draw(FR_MODULUS))
+    return create_proof_r1cs_batch(r1cs, params, inputs, aux, rs, ss, device_ptrs)

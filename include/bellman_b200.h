@@ -84,6 +84,7 @@ void bb_ctx_destroy(bb_ctx* ctx);
  *   msm_unified_rows_log   msm_precompute = 2: the rounds stop at about 2^this rows per bucket (default 3)
  *   msm_precompute_groups  which vectors use the tables: mask of 1 (G1) and 2 (G2), default 3
  *   shard_windows      multi-GPU: window groups per base range (default 4; 1 = base ranges only)
+ *   prove_batch_max    bb_groth16_prove_batch: at most this many proofs per sub-batch (0 = as many as memory allows)
  *   ntt_radix8         1 = register radix-8 NTT windows (default 0: measured slower), ntt_tile_log, ntt_col_bits
  *   profile            1 = CUDA-event timing of the MSM stages, and of the verify.*, decode.* and r1cs.* stages (bb_profile_read) */
 int bb_ctx_set_option(bb_ctx* ctx, const char* key, long value);
@@ -266,6 +267,24 @@ int bb_groth16_finalize_with(const bb_crs* crs, const uint8_t* partials, size_t 
  * b_g1_inputs, b_g1_aux, b_g2_inputs, b_g2_aux, h, l (:339-354). */
 int bb_groth16_prove(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w,
                      const uint8_t r[32], const uint8_t s[32], uint8_t proof[192]);
+/* create_proof (groth16/src/prover.rs:217-360) for `count` witnesses of ONE circuit against one key: w[i], r + 32 i and
+ * s + 32 i are what bb_groth16_prove takes, proof i goes to proofs + 192 i.  status[i] (written for every item whenever the call returns BB_OK) is exactly what
+ * bb_groth16_prove returns for item i alone -- the same codes in the same precedence -- and the proof bytes are its bytes;
+ * a failed item's 192 bytes are zero.  Returns BB_OK whenever the call ran, even if items failed (as bb_proofs_read).
+ * Every item must have item 0's n_constraints, n_inputs, n_aux and on_device and density words equal to item 0's (the
+ * circuit's structure decides them; the arrays may be distinct); otherwise BB_ERR_ARG naming the first differing item.
+ * BB_ERR_ARG also for NULL pointers with count > 0 and for a sharded key (shard_count > 1), before any device work.
+ * count = 0 is BB_OK and writes nothing.
+ * The call splits the batch into sub-batches by device memory and by the 2^32 bucket entries of one MSM job, at most
+ * bb_ctx_set_option(ctx, "prove_batch_max", k) proofs each (0 = no cap); the results never depend on the split.  A
+ * sub-batch whose buffers cannot be allocated gives its items BB_ERR_OOM; items of other sub-batches keep their proofs.
+ * A sub-batch runs one H pipeline per item and eight MSM jobs over all its items; r and s stay on the host (the ladder
+ * documented at bb_groth16_finalize_static), the scalar multiplications of the items run on a pool of host threads. */
+int bb_groth16_prove_batch(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t count,
+                           const uint8_t* r, const uint8_t* s, uint8_t* proofs, int* status);
+/* The message bb_last_error() holds after bb_groth16_prove returned `status` with this key: the text of a batch item's
+ * status.  NULL for back-end statuses (BB_ERR_ARG, _CUDA, _OOM), whose text depends on the failure. */
+const char* bb_groth16_prove_message(const bb_crs* crs, int status);
 
 /* ---- the constraint system on the device: ProvingAssignment::enforce (groth16/src/prover.rs:19-55,105-145) ---------
  * The A, B, C matrices of a circuit -- what KeypairAssembly records for generate_parameters (generator.rs:43-155) -- kept
@@ -309,6 +328,12 @@ int bb_r1cs_eval(bb_ctx* ctx, const bb_r1cs* r1cs, const void* input, size_t n_i
  * device work; then exactly bb_groth16_prove's errors and their precedence. */
 int bb_groth16_prove_r1cs(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* r1cs, const void* input, size_t n_inputs,
                           const void* aux, size_t n_aux, int on_device, const uint8_t r[32], const uint8_t s[32], uint8_t proof[192]);
+/* bb_groth16_prove_batch from witnesses alone: inputs = count x n_inputs Fr and aux = count x n_aux Fr, row-major (host, or
+ * device memory with on_device != 0).  status[i] and proof i are bb_groth16_prove_r1cs's for item i alone.  Argument errors
+ * as bb_r1cs_eval's and bb_groth16_prove_batch's, before any device work. */
+int bb_groth16_prove_r1cs_batch(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* r1cs, const void* inputs, size_t n_inputs,
+                                const void* aux, size_t n_aux, size_t count, int on_device, const uint8_t* r, const uint8_t* s,
+                                uint8_t* proofs, int* status);
 
 /* ---- verification: groth16/src/verifier.rs and groth16/src/verifier/batch.rs ------------------
  * Points are taken as valid curve and subgroup elements, as the reference's Proof / VerifyingKey types guarantee

@@ -167,6 +167,9 @@ extern "C" {
                                     static_in: *const u8, proof: *mut u8) -> c_int;
     pub fn bb_groth16_prove(ctx: *mut bb_ctx, crs: *const bb_crs, w: *const bb_witness, r: *const u8, s: *const u8,
                             proof: *mut u8) -> c_int;
+    pub fn bb_groth16_prove_message(crs: *const bb_crs, status: c_int) -> *const c_char;
+    pub fn bb_groth16_prove_batch(ctx: *mut bb_ctx, crs: *const bb_crs, w: *const bb_witness, count: usize, r: *const u8,
+                                  s: *const u8, proofs: *mut u8, status: *mut c_int) -> c_int;
     pub fn bb_r1cs_create(ctx: *mut bb_ctx, desc: *const bb_r1cs_desc, out: *mut *mut bb_r1cs) -> c_int;
     pub fn bb_r1cs_destroy(r1cs: *mut bb_r1cs);
     pub fn bb_r1cs_info(r1cs: *const bb_r1cs, shape: *mut u64, a_aux_density: *mut u64, b_input_density: *mut u64,
@@ -175,6 +178,9 @@ extern "C" {
                         n_aux: usize, in_on_device: c_int, a: *mut c_void, b: *mut c_void, c: *mut c_void, out_on_device: c_int) -> c_int;
     pub fn bb_groth16_prove_r1cs(ctx: *mut bb_ctx, crs: *const bb_crs, r1cs: *const bb_r1cs, input: *const c_void, n_inputs: usize,
                                  aux: *const c_void, n_aux: usize, on_device: c_int, r: *const u8, s: *const u8, proof: *mut u8) -> c_int;
+    pub fn bb_groth16_prove_r1cs_batch(ctx: *mut bb_ctx, crs: *const bb_crs, r1cs: *const bb_r1cs, inputs: *const c_void,
+                                       n_inputs: usize, aux: *const c_void, n_aux: usize, count: usize, on_device: c_int,
+                                       r: *const u8, s: *const u8, proofs: *mut u8, status: *mut c_int) -> c_int;
 
     pub fn bb_vk_prepare(ctx: *mut bb_ctx, desc: *const bb_vk_desc, out: *mut *mut bb_vk) -> c_int;
     pub fn bb_vk_destroy(vk: *mut bb_vk);

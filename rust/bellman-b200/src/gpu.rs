@@ -349,6 +349,52 @@ pub fn create_proof_b200(w: &WitnessView, crs: &GpuParameters, r: Scalar, s: Sca
     Proof::read(&bytes[..]).map_err(Into::into)               // the same 192 bytes Proof::write emits (lib.rs:39-45)
 }
 
+/// `create_proof_b200` for many witnesses of ONE circuit in one call (bb_groth16_prove_batch): one result per item, each
+/// exactly what `create_proof_b200` returns for that item alone.  `Err` only when the call itself was refused (witnesses of
+/// different shapes, a sharded key).
+pub fn create_proof_batch_b200(ws: &[WitnessView], crs: &GpuParameters, rs: &[Scalar], ss: &[Scalar])
+    -> Result<Vec<Result<Proof<Bls12>, SynthesisError>>, SynthesisError> {
+    assert!(rs.len() == ws.len() && ss.len() == ws.len(), "one r and one s per witness");
+    let wit: Vec<_> = ws.iter().map(|w| w.as_ffi()).collect();
+    batch_results(ws.len(), rs, ss, |r, s, proofs, st| unsafe {
+        bb_groth16_prove_batch(crs.ctx, crs.handle, wit.as_ptr(), ws.len(), r, s, proofs, st)
+    })
+}
+
+/// `create_proof_r1cs_b200` for many circuits of one shape (bb_groth16_prove_r1cs_batch): every circuit is synthesised
+/// with `WitnessCS` and the witnesses are proved in one call; one result per circuit.
+pub fn create_proof_r1cs_batch_b200<C: Circuit<Scalar>>(circuits: Vec<C>, r1cs: &GpuR1cs, crs: &GpuParameters, rs: &[Scalar], ss: &[Scalar])
+    -> Result<Vec<Result<Proof<Bls12>, SynthesisError>>, SynthesisError> {
+    let count = circuits.len();
+    assert!(rs.len() == count && ss.len() == count, "one r and one s per circuit");
+    let (mut inputs, mut aux) = (Vec::with_capacity(count * r1cs.n_inputs), Vec::with_capacity(count * r1cs.n_aux));
+    for circuit in circuits {
+        let mut cs = WitnessCS::default();
+        cs.alloc_input(|| "", || Ok(Scalar::one()))?;
+        circuit.synthesize(&mut cs)?;
+        assert_eq!((cs.input_assignment.len(), cs.aux_assignment.len()), (r1cs.n_inputs, r1cs.n_aux), "the circuit's shape changed");
+        inputs.extend(cs.input_assignment);
+        aux.extend(cs.aux_assignment);
+    }
+    batch_results(count, rs, ss, |r, s, proofs, st| unsafe {
+        bb_groth16_prove_r1cs_batch(crs.ctx, crs.handle, r1cs.handle, inputs.as_ptr() as _, r1cs.n_inputs, aux.as_ptr() as _, r1cs.n_aux,
+                                    count, 0, r, s, proofs, st)
+    })
+}
+
+/// the per-item statuses and 192-byte records of a batch call -> one `Result` per item
+fn batch_results(count: usize, rs: &[Scalar], ss: &[Scalar], call: impl FnOnce(*const u8, *const u8, *mut u8, *mut i32) -> i32)
+    -> Result<Vec<Result<Proof<Bls12>, SynthesisError>>, SynthesisError> {
+    let r: Vec<u8> = rs.iter().flat_map(|v| v.to_repr()).collect();
+    let s: Vec<u8> = ss.iter().flat_map(|v| v.to_repr()).collect();
+    let mut bytes = vec![0u8; 192 * count];
+    let mut st = vec![0i32; count];
+    status(call(r.as_ptr(), s.as_ptr(), bytes.as_mut_ptr(), st.as_mut_ptr()))?;
+    Ok(st.iter().zip(bytes.chunks(192))
+        .map(|(&rc, b)| status(rc).and_then(|_| Proof::read(b).map_err(Into::into)))
+        .collect())
+}
+
 /// `PreparedVerifyingKey` (groth16/src/lib.rs:400-409, verifier.rs:11-21): the verifying key resident on the device.
 pub struct GpuVerifyingKey { pub(crate) ctx: *mut bb_ctx, pub(crate) handle: *mut bb_vk, pub(crate) ic_len: usize }
 unsafe impl Send for GpuVerifyingKey {}
