@@ -444,15 +444,25 @@ class Parameters(_DeviceObject):
         d = _CrsDesc()
         d.alpha_g1, d.beta_g1, d.delta_g1 = (self._vk[i].ctypes.data for i in range(3))
         d.beta_g2, d.delta_g2 = self._vk[3].ctypes.data, self._vk[4].ctypes.data
+        self.lens = {"ic": int(np.asarray(p["ic"]).reshape(-1, 12).shape[0])} if "ic" in p else {}
         for name, width in (("h", 12), ("l", 12), ("a", 12), ("b_g1", 12), ("b_g2", 24)):
             arr = k[name].reshape(-1, width)
             setattr(d, name, arr.ctypes.data)
             setattr(d, name + "_len", arr.shape[0])
+            self.lens[name] = int(arr.shape[0])
         d.shard_index, d.shard_count = shard_index, shard_count
         h = C.c_void_p()
         _check(load_library().bb_crs_create(worker._h, C.byref(d), C.byref(h)))
         self._own(worker, h)
         self._keep = None                    # the vectors are resident in HBM now
+
+    @classmethod
+    def _from_handle(cls, worker, h, lens):
+        """a bb_crs built by the library itself (params_io.read_parameters_device); lens: the vector lengths"""
+        self = cls.__new__(cls)
+        self.worker, self._keep, self.lens = worker, None, dict(lens)
+        self._own(worker, h)
+        return self
 
     @classmethod
     def synthetic(cls, worker, seed, shape, shard_index=0, shard_count=1):
@@ -732,3 +742,5 @@ from .verifier import InvalidProofEncoding, read_proof, read_proofs, write_proof
 # the constraint system on the device: prove from the witness alone (groth16/src/prover.rs:19-55,105-145)
 from .r1cs import (R1CS, create_proof_r1cs, create_proof_r1cs_batch, create_random_proof_r1cs,  # noqa: E402
                    create_random_proof_r1cs_batch)
+# Parameters::read / VerifyingKey::read on the device (groth16/src/lib.rs:158-218, 289-398)
+from .params_io import InvalidData, read_parameters_device, read_verifying_key_device  # noqa: E402

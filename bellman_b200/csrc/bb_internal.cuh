@@ -87,6 +87,12 @@ struct bb_ctx {
     long opt_msm_precompute_groups = 3;  // which groups use the tables: bit 0 = G1 vectors, bit 1 = G2 vectors
     long opt_msm_unified_rows_log = 3;   // msm_precompute = 2: halving rounds until about 2^this rows per bucket are left
     long opt_prove_batch_max = 0;        // bb_groth16_prove_batch: at most this many proofs per sub-batch (0 = by memory)
+    long opt_params_read_chunk = 64l << 20;   // bb_params_read from host memory: staging bytes per chunk
+    // bb_params_read's two page-locked staging blocks (read_stage_bytes each), kept for the next read; read_mu serialises
+    // the reads that use them
+    std::mutex read_mu;
+    void* read_stage[2] = {nullptr, nullptr};
+    size_t read_stage_bytes = 0;
     struct ProfEntry { double ms = 0; uint64_t launches = 0, units = 0; };
     std::map<std::string, ProfEntry> prof;
     void prof_add(const char* what, double ms, uint64_t launches, uint64_t units) {
@@ -138,6 +144,7 @@ struct DevBuf {
     ~DevBuf() { reset(); }
     int alloc(bb_ctx* c, size_t bytes) { reset(); ctx = c; return c->alloc(bytes ? bytes : 16, &p); }
     void reset() { if (p && ctx) ctx->release(p); p = nullptr; }
+    void* take() { void* q = p; p = nullptr; return q; }      // the block now belongs to the caller
     template <class T> T* as() const { return (T*)p; }
 };
 
@@ -197,6 +204,14 @@ int prove_batch_impl(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t
                      uint8_t* proofs, int* status, const BatchAbcFill* fill = nullptr);
 int prove_batch_check(const char* fn, const bb_ctx* ctx, const bb_crs* crs, size_t count, const void* r, const void* s, const void* proofs,
                       const int* status);
+// A single-GPU bb_crs that adopts the five resident vectors h, l, a, b_g1, b_g2 (freed with it); g1 = alpha, beta, delta,
+// g2 = beta, delta (bb_params_read)
+bb_crs* crs_adopt(bb_ctx* ctx, bb_bases* const vec[5], const G1Affine g1[3], const G2Affine g2[2]);
+
+// ---- verify.cu ----
+// A bb_vk that adopts its device parts (context allocations): alpha_g1, the G2 points in the order delta, gamma, beta, and
+// the resident ic (bb_params_read, bb_vk_read)
+bb_vk* vk_adopt(bb_ctx* ctx, G1Affine* d_alpha, G2Affine* d_g2, bb_bases* ic);
 
 // ---- capi.cu ----
 int fixed_base_mul_device(bb_ctx* ctx, int group, const Fr* d_scalars, size_t n, bool montgomery, void* d_out, cudaStream_t st);

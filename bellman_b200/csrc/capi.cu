@@ -272,6 +272,7 @@ void bb_ctx_destroy(bb_ctx* ctx) {
     for (auto& kv : ctx->free_blocks) cudaFree(kv.second);
     for (auto& kv : ctx->live_blocks) cudaFree(kv.first);
     for (auto p : ctx->pinned_free) cudaFreeHost(p);
+    for (auto p : ctx->read_stage) if (p) cudaFreeHost(p);
     for (auto s : ctx->streams) cudaStreamDestroy(s);
     if (ctx->main_stream) cudaStreamDestroy(ctx->main_stream);
     for (auto& cs : ctx->crit_stream) if (cs) cudaStreamDestroy(cs);
@@ -294,6 +295,7 @@ int bb_ctx_set_option(bb_ctx* ctx, const char* key, long value) {
     else if (k == "msm_precompute_groups") { if (value < 0 || value > 3) { set_error("msm_precompute_groups is a mask of 1 (G1) and 2 (G2)"); return BB_ERR_ARG; } ctx->opt_msm_precompute_groups = value; }
     else if (k == "msm_unified_rows_log") { if (value < 0 || value > 12) { set_error("msm_unified_rows_log is 0..12"); return BB_ERR_ARG; } ctx->opt_msm_unified_rows_log = value; }
     else if (k == "prove_batch_max") { if (value < 0) { set_error("prove_batch_max >= 0"); return BB_ERR_ARG; } ctx->opt_prove_batch_max = value; }
+    else if (k == "params_read_chunk") { if (value < 1) { set_error("params_read_chunk >= 1"); return BB_ERR_ARG; } ctx->opt_params_read_chunk = value; }
     else if (k == "msm_affine_rounds") ctx->opt_msm_affine_rounds = value;
     else if (k == "msm_affine_batch") ctx->opt_msm_affine_batch = value;
     else if (k == "msm_affine_tma") ctx->opt_msm_affine_tma = value;
@@ -330,6 +332,13 @@ int bb_ctx_bytes_copied(const bb_ctx* ctx, uint64_t* h2d, uint64_t* d2h) {
     if (h2d) *h2d = ctx->h2d_bytes.load();
     if (d2h) *d2h = ctx->d2h_bytes.load();
     return BB_OK;
+}
+uint64_t bb_diag_ctx_live_bytes(const bb_ctx* ctx) {
+    if (!ctx) return 0;
+    std::lock_guard<std::mutex> g(const_cast<bb_ctx*>(ctx)->mu);
+    uint64_t s = 0;
+    for (auto& kv : ctx->live_blocks) s += kv.second;
+    return s;
 }
 int bb_profile_reset(bb_ctx* ctx) {
     if (!ctx) return BB_ERR_ARG;

@@ -23,6 +23,17 @@
 //   k_proof_status   folds the three element codes into the status byte, zeroes all points of an invalid proof
 //   k_encode_proofs  the inverse: Proof::write of n affine triples
 // Nothing outside this file calls into it.
+//
+// Parameters::read / VerifyingKey::read (groth16/src/lib.rs:158-218, 289-398) of a key file into a resident bb_crs / bb_vk:
+// the u32 length prefixes are walked on the host, every point is decoded on the device by
+//   k_params_decode_g1 / k_params_decode_g2   one thread per uncompressed point: flags, canonical coordinates,
+//                                             Montgomery form, curve equation and subgroup test (checked sections), the
+//                                             identity rule; the point goes straight to its index in the resident vector
+// and the first failure in file order is kept in one word, atomicMin((ordinal << 3) | why).  Host bytes are streamed in
+// chunks through two pinned staging blocks (copy of chunk k + 1 on a copy stream while chunk k decodes on the main
+// stream); device bytes are decoded in place.
+#include <cstring>
+
 #include "bb_internal.cuh"
 
 using namespace bb;
@@ -238,6 +249,320 @@ __global__ void __launch_bounds__(128) k_encode_proofs(const G1Affine* __restric
 
 constexpr size_t MAX_PROOFS = (size_t)1 << 31;
 
+// ---- Parameters::read: uncompressed points (from_uncompressed / _unchecked, then bellman's identity rule) ----------
+// why code of one point; *out = the Montgomery affine point (identity = zeros) when it is 0
+BB_D int g1_read_uncompressed(const uint8_t* s, bool checked, bool allow_identity, G1Affine* out) {
+    const uint32_t flags = s[0];
+    if (flags & 0xa0) return WHY_FLAGS;                                  // compression or sort bit
+    Fp x = fp_load_be(s, 0x1f), y = fp_load_be(s + 48, 0xff);
+    if (flags & 0x40) {
+        if (!x.is_zero() || !y.is_zero()) return WHY_FLAGS;
+        *out = G1Affine::identity();
+        return allow_identity ? WHY_OK : WHY_IDENTITY;
+    }
+    if (!fp_is_canonical(x) || !fp_is_canonical(y)) return WHY_NONCANONICAL;
+    G1Affine p{fp_from_canonical(x), fp_from_canonical(y)};
+    if (checked) {
+        if (p.y.sqr() != p.x.sqr() * p.x + g1_b()) return WHY_NOT_ON_CURVE;
+        if (!g1_in_subgroup(p)) return WHY_NOT_IN_SUBGROUP;
+    }
+    *out = p;
+    return WHY_OK;
+}
+BB_D int g2_read_uncompressed(const uint8_t* s, bool checked, bool allow_identity, G2Affine* out) {
+    const uint32_t flags = s[0];
+    if (flags & 0xa0) return WHY_FLAGS;
+    Fp x1 = fp_load_be(s, 0x1f), x0 = fp_load_be(s + 48, 0xff), y1 = fp_load_be(s + 96, 0xff), y0 = fp_load_be(s + 144, 0xff);
+    if (flags & 0x40) {
+        if (!x0.is_zero() || !x1.is_zero() || !y0.is_zero() || !y1.is_zero()) return WHY_FLAGS;
+        *out = G2Affine::identity();
+        return allow_identity ? WHY_OK : WHY_IDENTITY;
+    }
+    if (!fp_is_canonical(x0) || !fp_is_canonical(x1) || !fp_is_canonical(y0) || !fp_is_canonical(y1)) return WHY_NONCANONICAL;
+    G2Affine p{{fp_from_canonical(x0), fp_from_canonical(x1)}, {fp_from_canonical(y0), fp_from_canonical(y1)}};
+    if (checked) {
+        if (p.y.sqr() != p.x.sqr() * p.x + g2_b()) return WHY_NOT_ON_CURVE;
+        if (!g2_in_subgroup(p)) return WHY_NOT_IN_SUBGROUP;
+    }
+    *out = p;
+    return WHY_OK;
+}
+
+BB_D void first_failure(unsigned long long* first, unsigned long long code) {
+#if defined(__CUDACC__)
+    atomicMin(first, code);
+#else
+    unsigned long long old = __atomic_load_n(first, __ATOMIC_SEQ_CST);
+    while (old > code && !__atomic_compare_exchange_n(first, &old, code, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST)) {}
+#endif
+}
+
+// n points at src (stride 96 / 192) -> out[0 .. n); point i has ordinal ord0 + i in the file.  A point behind the first
+// failure seen so far is skipped: only the first failure in file order is reported.
+__global__ void __launch_bounds__(DECODE_THREADS) k_params_decode_g1(const uint8_t* __restrict__ src, size_t n, uint64_t ord0, int checked,
+                                                                     int allow_identity, G1Affine* out, unsigned long long* first) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const unsigned long long ord = ord0 + i;
+    if (*(volatile unsigned long long*)first < (ord << 3)) return;
+    G1Affine p;
+    int why = g1_read_uncompressed(src + i * 96, checked != 0, allow_identity != 0, &p);
+    if (why) first_failure(first, (ord << 3) | (unsigned)why);
+    else out[i] = p;
+}
+__global__ void __launch_bounds__(DECODE_THREADS) k_params_decode_g2(const uint8_t* __restrict__ src, size_t n, uint64_t ord0, int checked,
+                                                                     int allow_identity, G2Affine* out, unsigned long long* first) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const unsigned long long ord = ord0 + i;
+    if (*(volatile unsigned long long*)first < (ord << 3)) return;
+    G2Affine p;
+    int why = g2_read_uncompressed(src + i * 192, checked != 0, allow_identity != 0, &p);
+    if (why) first_failure(first, (ord << 3) | (unsigned)why);
+    else out[i] = p;
+}
+
+constexpr int PARAMS_SECTIONS = 12, VK_SECTIONS = 7;
+const char* const kSection[PARAMS_SECTIONS] = {"alpha_g1", "beta_g1", "beta_g2", "gamma_g2", "delta_g1", "delta_g2",
+                                               "ic", "h", "l", "a", "b_g1", "b_g2"};
+const char* const kWhy[6] = {"", "flag bits", "coordinate not below p", "not on the curve", "not in the prime-order subgroup", ""};
+bool section_g2(int s) { return s == BB_PARAMS_BETA_G2 || s == BB_PARAMS_GAMMA_G2 || s == BB_PARAMS_DELTA_G2 || s == BB_PARAMS_B_G2; }
+size_t point_bytes(int s) { return section_g2(s) ? 192 : 96; }
+
+// Where the sections of a key file lie, from its length prefixes: complete points only, so that nothing sized by a
+// prefix exceeds the buffer
+struct Layout {
+    int sections = 0;                      // sections reached (their complete points are decoded)
+    size_t off[PARAMS_SECTIONS] = {};      // byte offset of the section's first point
+    size_t count[PARAMS_SECTIONS] = {};    // complete points present
+    uint64_t ord0[PARAMS_SECTIONS] = {};   // ordinal of its first point in the file
+    size_t declared[6] = {};               // the six prefixes as read
+    bool eof = false;                      // the buffer ends inside the key: at eof_section, after eof_index of its points,
+    bool eof_prefix = false;               // (or inside its length prefix) at byte eof_offset
+    int eof_section = -1;
+    size_t eof_index = 0, eof_offset = 0;
+    size_t end = 0;                        // bytes of the key (complete keys)
+};
+
+int walk_layout(bb_ctx* ctx, const uint8_t* bytes, size_t len, bool on_device, int sections, Layout* L) {
+    size_t off = 0;
+    uint64_t ord = 0;
+    for (int s = 0; s < sections; s++) {
+        const size_t size = point_bytes(s);
+        size_t want = 1;
+        L->sections = s + 1;
+        if (s >= BB_PARAMS_IC) {
+            if (len - off < 4) { L->eof = L->eof_prefix = true; L->eof_section = s; L->eof_index = 0; L->eof_offset = off; L->sections = s; break; }
+            uint8_t b[4];
+            if (on_device) {
+                BB_CUDA(cudaMemcpy(b, bytes + off, 4, cudaMemcpyDeviceToHost));
+                ctx->d2h_bytes += 4;
+            } else {
+                std::memcpy(b, bytes + off, 4);
+            }
+            want = ((size_t)b[0] << 24) | ((size_t)b[1] << 16) | ((size_t)b[2] << 8) | b[3];
+            L->declared[s - BB_PARAMS_IC] = want;
+            off += 4;
+        }
+        const size_t have = (len - off) / size;
+        L->off[s] = off;
+        L->ord0[s] = ord;
+        L->count[s] = want < have ? want : have;
+        off += L->count[s] * size;
+        ord += L->count[s];
+        if (L->count[s] < want) { L->eof = true; L->eof_section = s; L->eof_index = L->count[s]; L->eof_offset = off; break; }
+    }
+    L->end = off;
+    return BB_OK;
+}
+
+// caller's host buffer in page-locked memory (then copied to the device without the staging memcpy)
+bool host_pinned(const void* p, size_t len) {
+#if defined(__CUDACC__)
+    for (const void* q : {p, (const void*)((const uint8_t*)p + len - 1)}) {
+        cudaPointerAttributes a;
+        if (cudaPointerGetAttributes(&a, q) != cudaSuccess) { cudaGetLastError(); return false; }
+        if (a.type != cudaMemoryTypeHost) return false;
+    }
+    return true;
+#else
+    (void)p; (void)len;
+    return false;
+#endif
+}
+
+struct Events {                           // destroyed with the call
+    cudaEvent_t e[4] = {nullptr, nullptr, nullptr, nullptr};
+    ~Events() { for (auto x : e) if (x) cudaEventDestroy(x); }
+};
+
+int params_read_impl(bb_ctx* ctx, const void* bytes, size_t len, int on_device, int checked, int sections, bb_crs** crs_out,
+                     bb_vk** vk_out, bb_params_report* report) {
+    const char* fn = sections == PARAMS_SECTIONS ? "bb_params_read" : "bb_vk_read";
+    if (crs_out) *crs_out = nullptr;
+    if (vk_out) *vk_out = nullptr;
+    bb_params_report rep{};
+    rep.section = -1;
+    if (report) *report = rep;
+    if (!ctx || (len && !bytes) || (sections == PARAMS_SECTIONS ? !crs_out : !vk_out)) {
+        set_error("%s: null argument", fn);
+        return BB_ERR_ARG;
+    }
+    BB_CUDA(cudaSetDevice(ctx->device));
+    NvtxRange nvtx("params_read");
+    const uint8_t* src = (const uint8_t*)bytes;
+    Layout L;
+    BB_TRY(walk_layout(ctx, src, len, on_device != 0, sections, &L));
+    for (int k = 0; k < 6; k++) rep.len[k] = L.declared[k];
+
+    // destinations at their final size (complete points only): alpha; beta_g1, delta_g1; the G2 points in bb_vk's order
+    // delta, gamma, beta; ic; the five vectors
+    DevBuf d_alpha, d_g1x, d_g2, d_vec[6], d_first;
+    BB_TRY(d_alpha.alloc(ctx, sizeof(G1Affine)));
+    BB_TRY(d_g1x.alloc(ctx, 2 * sizeof(G1Affine)));
+    BB_TRY(d_g2.alloc(ctx, 3 * sizeof(G2Affine)));
+    for (int k = 0; k < sections - BB_PARAMS_IC; k++) {
+        const int s = BB_PARAMS_IC + k;
+        BB_TRY(d_vec[k].alloc(ctx, (L.count[s] ? L.count[s] : 1) * point_bytes(s)));
+    }
+    BB_TRY(d_first.alloc(ctx, 8));
+    void* dest[PARAMS_SECTIONS] = {d_alpha.p, d_g1x.p, d_g2.as<G2Affine>() + 2, d_g2.as<G2Affine>() + 1, d_g1x.as<G1Affine>() + 1, d_g2.p};
+    for (int k = 0; k < sections - BB_PARAMS_IC; k++) dest[BB_PARAMS_IC + k] = d_vec[k].p;
+
+    cudaStream_t st = ctx->main_stream;
+    // host input: device staging blocks, events and the pinned blocks' lock live until the stream is drained below
+    DevBuf d_stage[2];
+    Events ev;                                                    // copied[b], decoded[b]
+    std::unique_lock<std::mutex> stage_lock(ctx->read_mu, std::defer_lock);
+    StageTimer tm(ctx, st);
+    tm.mark("params.begin");
+    BB_CUDA(cudaMemsetAsync(d_first.p, 0xff, 8, st));
+    unsigned long long* first = d_first.as<unsigned long long>();
+    uint64_t points = 0;
+    auto launch = [&](int s, const uint8_t* p, size_t lo, size_t n) {
+        const int chk = s <= BB_PARAMS_IC || checked ? 1 : 0, allow = s < BB_PARAMS_IC ? 1 : 0;
+        const uint64_t ord = L.ord0[s] + lo;
+        if (section_g2(s))
+            k_params_decode_g2<<<cdiv(n, DECODE_THREADS), DECODE_THREADS, 0, st>>>(p, n, ord, chk, allow, (G2Affine*)dest[s] + lo, first);
+        else
+            k_params_decode_g1<<<cdiv(n, DECODE_THREADS), DECODE_THREADS, 0, st>>>(p, n, ord, chk, allow, (G1Affine*)dest[s] + lo, first);
+        ctx->count_launch();
+        tm.mark(section_g2(s) ? "params.g2" : "params.g1");
+        points += n;
+    };
+
+    if (on_device) {                                              // in place: one launch per section
+        for (int s = 0; s < L.sections; s++)
+            if (L.count[s]) launch(s, src + L.off[s], 0, L.count[s]);
+        BB_CUDA(cudaGetLastError());
+    } else if (L.end) {
+        // chunks of whole points; chunk k is copied into device block k % 2 on the copy stream while chunk k - 1 decodes
+        const size_t chunk = (size_t)ctx->opt_params_read_chunk;
+        const size_t cap = chunk < 192 ? 192 : chunk;             // one point at least
+        const bool direct = host_pinned(bytes, len);
+        if (!direct) {
+            stage_lock.lock();
+            if (ctx->read_stage_bytes < cap) {
+                for (auto& p : ctx->read_stage) { if (p) cudaFreeHost(p); p = nullptr; }
+                ctx->read_stage_bytes = 0;
+                for (auto& p : ctx->read_stage) BB_CUDA(cudaMallocHost(&p, cap));
+                ctx->read_stage_bytes = cap;
+            }
+        }
+        BB_TRY(d_stage[0].alloc(ctx, cap));
+        BB_TRY(d_stage[1].alloc(ctx, cap));
+        for (auto& e : ev.e) BB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        cudaEvent_t* copied = ev.e;
+        cudaEvent_t* decoded = ev.e + 2;
+        cudaStream_t cp = ctx->pick_stream();
+        size_t k = 0;
+        for (int s = 0; s < L.sections; s++) {
+            const size_t size = point_bytes(s), per = chunk / size ? chunk / size : 1;
+            for (size_t lo = 0; lo < L.count[s]; lo += per, k++) {
+                const size_t n = L.count[s] - lo < per ? L.count[s] - lo : per, nb = n * size;
+                const int b = (int)(k & 1);
+                const uint8_t* h = src + L.off[s] + lo * size;
+                if (k >= 2) BB_CUDA(cudaStreamWaitEvent(cp, decoded[b], 0));     // chunk k - 2 has left block b
+                if (!direct) {
+                    if (k >= 2) BB_CUDA(cudaEventSynchronize(copied[b]));        // ... and its pinned block
+                    std::memcpy(ctx->read_stage[b], h, nb);
+                    h = (const uint8_t*)ctx->read_stage[b];
+                }
+                BB_CUDA(cudaMemcpyAsync(d_stage[b].p, h, nb, cudaMemcpyHostToDevice, cp));
+                ctx->h2d_bytes += nb;
+                BB_CUDA(cudaEventRecord(copied[b], cp));
+                BB_CUDA(cudaStreamWaitEvent(st, copied[b], 0));
+                tm.mark("params.upload");
+                launch(s, d_stage[b].as<uint8_t>(), lo, n);
+                BB_CUDA(cudaEventRecord(decoded[b], st));
+            }
+        }
+        BB_CUDA(cudaGetLastError());
+        // every copy is behind an event the main stream waited for: draining it drains the copy stream's work too
+    }
+    unsigned long long bad = ~0ull;
+    BB_CUDA(cudaMemcpyAsync(&bad, first, 8, cudaMemcpyDeviceToHost, st));
+    G1Affine g1[3];
+    G2Affine g2[3];                                               // delta, gamma, beta
+    BB_CUDA(cudaMemcpyAsync(&g1[0], d_alpha.p, sizeof(G1Affine), cudaMemcpyDeviceToHost, st));
+    BB_CUDA(cudaMemcpyAsync(&g1[1], d_g1x.p, 2 * sizeof(G1Affine), cudaMemcpyDeviceToHost, st));
+    BB_CUDA(cudaMemcpyAsync(g2, d_g2.p, sizeof g2, cudaMemcpyDeviceToHost, st));
+    BB_CUDA(cudaStreamSynchronize(st));
+    tm.report(points);
+
+    if (bad != ~0ull) {                                           // the first invalid point in file order
+        const uint64_t ord = bad >> 3;
+        const int why = (int)(bad & 7);
+        int s = 0;
+        while (s + 1 < L.sections && ord >= L.ord0[s + 1]) s++;
+        rep.section = s;
+        rep.index = (size_t)(ord - L.ord0[s]);
+        rep.why = why;
+        rep.consumed = L.off[s] + rep.index * point_bytes(s);
+        if (s < BB_PARAMS_IC) {
+            if (why == WHY_IDENTITY) set_error("%s: point at infinity", kSection[s]);
+            else set_error("%s: invalid %s (%s)", kSection[s], section_g2(s) ? "G2" : "G1", kWhy[why]);
+        } else {
+            if (why == WHY_IDENTITY) set_error("%s[%zu]: point at infinity", kSection[s], rep.index);
+            else set_error("%s[%zu]: invalid %s (%s)", kSection[s], rep.index, section_g2(s) ? "G2" : "G1", kWhy[why]);
+        }
+        if (report) *report = rep;
+        return BB_ERR_IO_INVALID_DATA;
+    }
+    if (L.eof) {
+        rep.section = L.eof_section;
+        rep.index = L.eof_index;
+        rep.consumed = L.eof_offset;
+        if (L.eof_section < BB_PARAMS_IC)
+            set_error("%s: unexpected end of file (failed to fill whole buffer)", kSection[L.eof_section]);
+        else if (L.eof_prefix)
+            set_error("%s: unexpected end of file in the length prefix (failed to fill whole buffer)", kSection[L.eof_section]);
+        else
+            set_error("%s[%zu]: unexpected end of file (failed to fill whole buffer)", kSection[L.eof_section], L.eof_index);
+        if (report) *report = rep;
+        return BB_ERR_IO_UNEXPECTED_EOF;
+    }
+
+    rep.consumed = L.end;
+    auto bases = [&](int s) {
+        bb_bases* b = new bb_bases();
+        b->ctx = ctx; b->group = section_g2(s) ? BB_G2 : BB_G1; b->n = L.count[s]; b->global_offset = 0; b->global_len = L.count[s];
+        b->d_points = d_vec[s - BB_PARAMS_IC].take();
+        return b;
+    };
+    bb_bases* ic = vk_out ? bases(BB_PARAMS_IC) : nullptr;
+    if (crs_out) {
+        bb_bases* vec[5];
+        for (int k = 0; k < 5; k++) vec[k] = bases(BB_PARAMS_H + k);
+        const G1Affine vg1[3] = {g1[0], g1[1], g1[2]};
+        const G2Affine vg2[2] = {g2[2], g2[0]};
+        *crs_out = crs_adopt(ctx, vec, vg1, vg2);
+    }
+    if (vk_out) *vk_out = vk_adopt(ctx, (G1Affine*)d_alpha.take(), (G2Affine*)d_g2.take(), ic);
+    if (report) *report = rep;
+    return BB_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -360,6 +685,15 @@ int bb_diag_points_decompress(bb_ctx* ctx, int group, const void* bytes, size_t 
     BB_CUDA(cudaMemcpyAsync(why, d_why.p, n, cudaMemcpyDeviceToHost, st));
     BB_CUDA(cudaStreamSynchronize(st));
     return BB_OK;
+}
+
+int bb_params_read(bb_ctx* ctx, const void* bytes, size_t len, int on_device, int checked, bb_crs** crs_out, bb_vk** vk_out,
+                   bb_params_report* report) {
+    return params_read_impl(ctx, bytes, len, on_device, checked, PARAMS_SECTIONS, crs_out, vk_out, report);
+}
+
+int bb_vk_read(bb_ctx* ctx, const void* bytes, size_t len, int on_device, bb_vk** vk_out, bb_params_report* report) {
+    return params_read_impl(ctx, bytes, len, on_device, 1, VK_SECTIONS, nullptr, vk_out, report);
 }
 
 }  // extern "C"

@@ -201,7 +201,34 @@ void bb_crs_destroy(bb_crs* crs) {
     delete crs;
 }
 
+int bb_diag_crs_download(const bb_crs* crs, int which, void* out) {
+    if (!crs || !out || which < 0 || which > 5) { set_error("bb_diag_crs_download: bad argument"); return BB_ERR_ARG; }
+    if (which == 5) {
+        uint8_t* o = (uint8_t*)out;
+        std::memcpy(o, &crs->alpha_g1, 96); std::memcpy(o + 96, &crs->beta_g1, 96); std::memcpy(o + 192, &crs->delta_g1, 96);
+        std::memcpy(o + 288, &crs->beta_g2, 192); std::memcpy(o + 480, &crs->delta_g2, 192);
+        return BB_OK;
+    }
+    const bb_bases* b = which == 0 ? crs->h : which == 1 ? crs->l : which == 2 ? crs->a : which == 3 ? crs->b_g1 : crs->b_g2;
+    const size_t bytes = b->n * (b->group == BB_G1 ? sizeof(G1Affine) : sizeof(G2Affine));
+    BB_CUDA(cudaSetDevice(crs->ctx->device));
+    if (bytes) BB_CUDA(cudaMemcpyAsync(out, b->d_points, bytes, cudaMemcpyDeviceToHost, crs->ctx->main_stream));
+    BB_CUDA(cudaStreamSynchronize(crs->ctx->main_stream));
+    return BB_OK;
+}
+
 }  // extern "C"
+
+namespace bb {
+bb_crs* crs_adopt(bb_ctx* ctx, bb_bases* const vec[5], const G1Affine g1[3], const G2Affine g2[2]) {
+    bb_crs* crs = new bb_crs();
+    crs->ctx = ctx;
+    crs->h = vec[0]; crs->l = vec[1]; crs->a = vec[2]; crs->b_g1 = vec[3]; crs->b_g2 = vec[4];
+    crs->alpha_g1 = g1[0]; crs->beta_g1 = g1[1]; crs->delta_g1 = g1[2];
+    crs->beta_g2 = g2[0]; crs->delta_g2 = g2[1];
+    return crs;
+}
+}  // namespace bb
 
 namespace {
 

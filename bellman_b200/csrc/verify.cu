@@ -612,6 +612,22 @@ int bb_vk_prepare(bb_ctx* ctx, const bb_vk_desc* d, bb_vk** out) {
     return BB_OK;
 }
 
+}  // extern "C"
+
+namespace bb {
+bb_vk* vk_adopt(bb_ctx* ctx, G1Affine* d_alpha, G2Affine* d_g2, bb_bases* ic) {
+    bb_vk* vk = new bb_vk();
+    vk->ctx = ctx;
+    vk->d_alpha = d_alpha;
+    vk->d_g2 = d_g2;
+    vk->ic = ic;
+    vk->ic_len = ic->n;
+    return vk;
+}
+}  // namespace bb
+
+extern "C" {
+
 void bb_vk_destroy(bb_vk* vk) {
     if (!vk) return;
     if (vk->d_alpha) vk->ctx->release(vk->d_alpha);

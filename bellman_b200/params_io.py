@@ -20,13 +20,19 @@ limbs, identity = all-zero) and applies the reference's acceptance rules:
   (lib.rs:294-298,328-332).  This is curve arithmetic, so it runs on the device
   (`bb_points_validate`): pass the `Worker` to use, or one is created on device 0 -- without a CUDA
   device the call fails, there is no CPU fallback.
+
+`read_parameters_device` / `read_verifying_key_device` read the same files on the device
+(`bb_params_read` / `bb_vk_read`): the bytes are decoded and checked there, straight into a
+resident `Parameters` (and `PreparedVerifyingKey`), with no host arrays.  They follow
+Parameters::read / VerifyingKey::read exactly, point by point: the first failing point in file
+order decides, and a short file is EOF only when every complete point before its end is valid.
 """
 import ctypes as C
 import struct
 
 import numpy as np
 
-from . import _check, load_library
+from . import _addr, _check, _ERRORS, load_library
 
 
 def _coords_to_abi(raw, ncoord, g2):
@@ -57,7 +63,17 @@ def _abi_to_coords(limbs, ncoord, g2):
 
 
 class InvalidData(ValueError):
-    """io::ErrorKind::InvalidData of Parameters::read / VerifyingKey::read"""
+    """io::ErrorKind::InvalidData of Parameters::read / VerifyingKey::read.  From the device reader: `section` (its name,
+    e.g. "h"), `index` within it and `why` (BB_READ_* code: 1 flags, 2 coordinate >= p, 3 off the curve, 4 outside the
+    subgroup, 5 identity)."""
+
+    def __init__(self, message, section=None, index=None, why=None):
+        super().__init__(message)
+        self.section, self.index, self.why = section, index, why
+
+
+BB_ERR_IO_INVALID_DATA = 8
+_ERRORS[BB_ERR_IO_INVALID_DATA] = InvalidData
 
 
 def _read_points(buf, off, count, g2, what, allow_infinity, validate):
@@ -159,6 +175,77 @@ def read_parameters(data, checked=True, worker=None):
     finally:
         val.close()
     return p
+
+
+SECTIONS = ("alpha_g1", "beta_g1", "beta_g2", "gamma_g2", "delta_g1", "delta_g2", "ic", "h", "l", "a", "b_g1", "b_g2")
+
+
+class ParamsReport(C.Structure):
+    """bb_params_report"""
+    _fields_ = [("len", C.c_size_t * 6), ("consumed", C.c_size_t), ("section", C.c_int), ("index", C.c_size_t), ("why", C.c_int)]
+
+
+def _device_read(worker, data, checked, want_crs, want_vk):
+    """bb_params_read (want_crs) or bb_vk_read of `data` -> (crs handle, vk handle, report); raises InvalidData / EOFError"""
+    lib = load_library()
+    keep = None
+    if isinstance(data, tuple):                                   # (device pointer, length): bytes in HBM
+        ptr, n, on_device = _addr(data[0]), int(data[1]), 1
+    else:
+        keep = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, np.uint8).reshape(-1)
+        ptr, n, on_device = (keep.ctypes.data if keep.size else None), keep.size, 0
+    rep = ParamsReport()
+    crs, vk = C.c_void_p(), C.c_void_p()
+    if want_crs:
+        rc = lib.bb_params_read(worker._h, C.c_void_p(ptr), C.c_size_t(n), C.c_int(on_device), C.c_int(1 if checked else 0), C.byref(crs),
+                                C.byref(vk) if want_vk else None, C.byref(rep))
+    else:
+        rc = lib.bb_vk_read(worker._h, C.c_void_p(ptr), C.c_size_t(n), C.c_int(on_device), C.byref(vk), C.byref(rep))
+    if rc == BB_ERR_IO_INVALID_DATA:
+        raise InvalidData(lib.bb_last_error().decode(errors="replace"), section=SECTIONS[rep.section], index=int(rep.index), why=int(rep.why))
+    if rc == 3:                                                   # BB_ERR_IO_UNEXPECTED_EOF
+        raise EOFError(lib.bb_last_error().decode(errors="replace"))
+    _check(rc)
+    return crs, vk, rep
+
+
+def read_parameters_device(worker, data, checked=True, verifying_key=False):
+    """Parameters::read(reader, checked) on the device (bb_params_read) -> a resident Parameters, or with
+    verifying_key=True (Parameters, PreparedVerifyingKey).  data: bytes, bytearray, memoryview or a uint8 array (host,
+    pageable or pinned), or (device_ptr, length) for bytes in HBM.  Bytes after the key are not read.  Raises InvalidData
+    (with .section, .index, .why) or EOFError as read_parameters does, in the reference's precedence."""
+    from . import Parameters
+    from .verifier import PreparedVerifyingKey
+    crs, vk, rep = _device_read(worker, data, checked, True, verifying_key)
+    lens = dict(zip(("ic", "h", "l", "a", "b_g1", "b_g2"), (int(v) for v in rep.len)))
+    params = Parameters._from_handle(worker, crs, lens)
+    if not verifying_key:
+        return params
+    return params, PreparedVerifyingKey._from_handle(worker, vk, lens["ic"])
+
+
+def read_verifying_key_device(worker, data):
+    """VerifyingKey::read + prepare_verifying_key on the device (bb_vk_read) -> (PreparedVerifyingKey, bytes consumed).
+    data as for read_parameters_device; a Parameters file starts with its VerifyingKey."""
+    from .verifier import PreparedVerifyingKey
+    _, vk, rep = _device_read(worker, data, True, False, True)
+    return PreparedVerifyingKey._from_handle(worker, vk, int(rep.len[0])), int(rep.consumed)
+
+
+def download_parameters(params):
+    """diagnostic (bb_diag_crs_download): the points a resident Parameters holds, as the dict read_parameters returns
+    (without gamma_g2 and ic, which bb_crs does not keep): vk_g1 (alpha, beta, delta), vk_g2 (beta, delta), h, l, a,
+    b_g1, b_g2"""
+    lib = load_library()
+    out = {}
+    for which, (name, width) in enumerate((("h", 12), ("l", 12), ("a", 12), ("b_g1", 12), ("b_g2", 24))):
+        arr = np.zeros((max(params.lens[name], 1), width), np.uint64)
+        _check(lib.bb_diag_crs_download(params._h, C.c_int(which), arr.ctypes.data_as(C.c_void_p)))
+        out[name] = arr[:params.lens[name]]
+    vk = np.zeros(3 * 12 + 2 * 24, np.uint64)
+    _check(lib.bb_diag_crs_download(params._h, C.c_int(5), vk.ctypes.data_as(C.c_void_p)))
+    out["vk_g1"], out["vk_g2"] = vk[:36].reshape(3, 12), vk[36:].reshape(2, 24)
+    return out
 
 
 def write_parameters(p):

@@ -71,6 +71,15 @@ class PreparedVerifyingKey(_DeviceObject):
         self._own(worker, h)
 
 
+    @classmethod
+    def _from_handle(cls, worker, h, ic_len):
+        """a bb_vk built by the library itself (params_io.read_parameters_device / read_verifying_key_device)"""
+        self = cls.__new__(cls)
+        self.worker, self.ic_len = worker, int(ic_len)
+        self._own(worker, h)
+        return self
+
+
 def prepare_verifying_key(worker, vk):
     """verifier.rs:11-21"""
     return PreparedVerifyingKey(worker, vk)

@@ -43,6 +43,7 @@ typedef enum bb_status {
     /* VerificationError (src/lib.rs:353-358) */
     BB_ERR_INVALID_VERIFYING_KEY = 6,       /* inputs.len() + 1 != ic.len(): verifier.rs:28-30, batch.rs:105-111 */
     BB_ERR_INVALID_PROOF = 7,               /* the pairing equation does not hold */
+    BB_ERR_IO_INVALID_DATA = 8,             /* io::ErrorKind::InvalidData of Parameters::read / VerifyingKey::read */
     /* back-end errors */
     BB_ERR_ARG = 16,
     BB_ERR_CUDA = 17,
@@ -85,8 +86,11 @@ void bb_ctx_destroy(bb_ctx* ctx);
  *   msm_precompute_groups  which vectors use the tables: mask of 1 (G1) and 2 (G2), default 3
  *   shard_windows      multi-GPU: window groups per base range (default 4; 1 = base ranges only)
  *   prove_batch_max    bb_groth16_prove_batch: at most this many proofs per sub-batch (0 = as many as memory allows)
+ *   params_read_chunk  bb_params_read / bb_vk_read from host memory: staging bytes per chunk (default 64 MiB; rounded
+ *                      down to whole points, at least one point)
  *   ntt_radix8         1 = register radix-8 NTT windows (default 0: measured slower), ntt_tile_log, ntt_col_bits
- *   profile            1 = CUDA-event timing of the MSM stages, and of the verify.*, decode.* and r1cs.* stages (bb_profile_read) */
+ *   profile            1 = CUDA-event timing of the MSM stages, and of the verify.*, decode.*, r1cs.* and params.* stages
+ *                      (bb_profile_read) */
 int bb_ctx_set_option(bb_ctx* ctx, const char* key, long value);
 int bb_ctx_synchronize(bb_ctx* ctx);
 /* counters for the harness: number of kernels this context has launched */
@@ -406,6 +410,44 @@ int bb_proofs_read(bb_ctx* ctx, const bb_proof_bytes* in, void* a, void* b, void
 /* Proof::write (lib.rs:39-45) over n proofs: out = n x 192 B (a, b, c and out are device pointers if on_device).
  * Byte for byte what bb_point_compress gives for each point. */
 int bb_proofs_write(bb_ctx* ctx, const void* a, const void* b, const void* c, size_t n, int on_device, void* out);
+
+/* ---- reading keys: Parameters::read / VerifyingKey::read (groth16/src/lib.rs:158-218, 289-398) -----------------------
+ * A key file is read once and decoded on the device, straight into a resident bb_crs (and bb_vk).  File order, all
+ * integers big-endian u32: alpha_g1, beta_g1, beta_g2, gamma_g2, delta_g1, delta_g2, |ic|, ic, then (Parameters only)
+ * |h|, h, |l|, l, |a|, a, |b_g1|, b_g1, |b_g2|, b_g2.  Points are uncompressed ZCash encodings (G1 96 B: x | y; G2
+ * 192 B: x.c1 | x.c0 | y.c1 | y.c0).  Each point is checked in this order; the first failing check gives its why code
+ * (the BB_READ_* values of bb_proofs_read):
+ *     1  compression (0x80) or sort (0x20) bit set, or the infinity bit (0x40) with any other bit of the point set
+ *     2  a coordinate >= p
+ *     3  not on the curve                  } only in checked sections: the six VerifyingKey points and ic always,
+ *     4  not in the order-r subgroup       } h, l, a, b_g1, b_g2 when checked != 0
+ *     5  the identity where it is not allowed: in ic and the five vectors (both modes); the six VerifyingKey points may be
+ *        the identity (the prover reports delta = identity itself)
+ * The first failing point in file order decides, as the reference reads point by point: BB_ERR_IO_INVALID_DATA, with
+ * bb_last_error() = "<section>[<index>]: invalid G1 (<reason>)" / "... invalid G2 ..." / "...: point at infinity".
+ * Only when every complete point before the end of the buffer is valid does a short buffer (a truncated point, a
+ * truncated prefix, a prefix claiming more points than the buffer holds) give BB_ERR_IO_UNEXPECTED_EOF.  Nothing is
+ * allocated beyond what the buffer can hold.  Bytes after the key are not read.  On failure *crs_out and *vk_out are
+ * NULL and everything the call allocated is back in the context's cache.
+ * bytes: host memory (pageable or pinned; streamed through two pinned staging blocks, copies overlapping the decode) or,
+ * with on_device != 0, device memory (decoded in place).  The result is what bb_crs_create / bb_vk_prepare build from the
+ * same points.  Single GPU keys only (shard 0 of 1).  BB_ERR_ARG, before any device work: a NULL ctx or out pointer, a
+ * NULL bytes with len > 0. */
+enum { BB_PARAMS_ALPHA_G1 = 0, BB_PARAMS_BETA_G1, BB_PARAMS_BETA_G2, BB_PARAMS_GAMMA_G2, BB_PARAMS_DELTA_G1,
+       BB_PARAMS_DELTA_G2, BB_PARAMS_IC, BB_PARAMS_H, BB_PARAMS_L, BB_PARAMS_A, BB_PARAMS_B_G1, BB_PARAMS_B_G2 };
+typedef struct bb_params_report {
+    size_t len[6];      /* ic, h, l, a, b_g1, b_g2 as their prefixes declared them (0 for prefixes not reached) */
+    size_t consumed;    /* bytes read: the key's length on success; on EOF the offset of the incomplete element */
+    int section;        /* first failing element (BB_PARAMS_*), -1 if none */
+    size_t index;       /* its index within the section; on EOF the number of complete points of that section */
+    int why;            /* BB_READ_* 1..5 for invalid data; 0 otherwise */
+} bb_params_report;
+/* Parameters::read(reader, checked): *crs_out = the proving key; vk_out (may be NULL) = its PreparedVerifyingKey too;
+ * report may be NULL */
+int bb_params_read(bb_ctx* ctx, const void* bytes, size_t len, int on_device, int checked,
+                   bb_crs** crs_out, bb_vk** vk_out, bb_params_report* report);
+/* VerifyingKey::read + prepare_verifying_key: the first 868 + 96 |ic| bytes of a VerifyingKey or Parameters file */
+int bb_vk_read(bb_ctx* ctx, const void* bytes, size_t len, int on_device, bb_vk** vk_out, bb_params_report* report);
 
 /* ---- tuning per key ------------------------------------------------------------------------
  * The MSM has several forms with identical results (per-window bucket sets; one bucket set over resident window

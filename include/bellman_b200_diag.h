@@ -76,6 +76,14 @@ int bb_synth_proof_batch(bb_ctx* ctx, uint64_t seed, size_t n, size_t n_inputs, 
  * bytes, the codes of bb_proofs_read (5 = the identity, a valid encoding that Proof::read rejects). */
 int bb_diag_points_decompress(bb_ctx* ctx, int group, const void* bytes, size_t n, int check_subgroup, void* out, uint8_t* why);
 
+/* ---- resident keys (prover.cu, capi.cu) ------------------------------------------------------------------------ */
+/* the points a bb_crs holds, ABI format, to host memory: which 0..4 = h, l, a, b_g1, b_g2 (the points this key holds of
+ * that vector: all of them on a single GPU); which 5 = alpha_g1, beta_g1, delta_g1 (96 B each) then beta_g2, delta_g2
+ * (192 B each) */
+int bb_diag_crs_download(const bb_crs* crs, int which, void* out);
+/* bytes of device memory the context has handed out and not yet taken back (its cache of free blocks excluded) */
+uint64_t bb_diag_ctx_live_bytes(const bb_ctx* ctx);
+
 #ifdef __cplusplus
 }
 #endif

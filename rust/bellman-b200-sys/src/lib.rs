@@ -21,6 +21,7 @@ pub const BB_ERR_IO_UNEXPECTED_EOF: c_int = 3;
 pub const BB_ERR_DENSITY_MISMATCH: c_int = 5;
 pub const BB_ERR_INVALID_VERIFYING_KEY: c_int = 6;
 pub const BB_ERR_INVALID_PROOF: c_int = 7;
+pub const BB_ERR_IO_INVALID_DATA: c_int = 8;
 pub const BB_ERR_ARG: c_int = 16;
 pub const BB_ERR_CUDA: c_int = 17;
 pub const BB_ERR_NO_DEVICE: c_int = 18;
@@ -100,6 +101,26 @@ pub const BB_READ_IDENTITY: u8 = 5;
 #[repr(C)]
 pub struct bb_proof_bytes {
     pub bytes: *const c_void, pub n: usize, pub stride: usize, pub on_device: c_int,
+}
+
+// key files: the sections of Parameters::read in file order, and what bb_params_read / bb_vk_read report
+pub const BB_PARAMS_ALPHA_G1: c_int = 0;
+pub const BB_PARAMS_BETA_G1: c_int = 1;
+pub const BB_PARAMS_BETA_G2: c_int = 2;
+pub const BB_PARAMS_GAMMA_G2: c_int = 3;
+pub const BB_PARAMS_DELTA_G1: c_int = 4;
+pub const BB_PARAMS_DELTA_G2: c_int = 5;
+pub const BB_PARAMS_IC: c_int = 6;
+pub const BB_PARAMS_H: c_int = 7;
+pub const BB_PARAMS_L: c_int = 8;
+pub const BB_PARAMS_A: c_int = 9;
+pub const BB_PARAMS_B_G1: c_int = 10;
+pub const BB_PARAMS_B_G2: c_int = 11;
+
+#[repr(C)]
+#[derive(Default)]
+pub struct bb_params_report {
+    pub len: [usize; 6], pub consumed: usize, pub section: c_int, pub index: usize, pub why: c_int,
 }
 
 extern "C" {
@@ -193,6 +214,10 @@ extern "C" {
                           out_on_device: c_int, status: *mut u8, n_invalid: *mut usize) -> c_int;
     pub fn bb_proofs_write(ctx: *mut bb_ctx, a: *const c_void, b: *const c_void, c: *const c_void, n: usize, on_device: c_int,
                            out: *mut c_void) -> c_int;
+    pub fn bb_params_read(ctx: *mut bb_ctx, bytes: *const c_void, len: usize, on_device: c_int, checked: c_int,
+                          crs_out: *mut *mut bb_crs, vk_out: *mut *mut bb_vk, report: *mut bb_params_report) -> c_int;
+    pub fn bb_vk_read(ctx: *mut bb_ctx, bytes: *const c_void, len: usize, on_device: c_int, vk_out: *mut *mut bb_vk,
+                      report: *mut bb_params_report) -> c_int;
 
     pub fn bb_tuning_count() -> c_int;
     pub fn bb_tuning_name(index: c_int) -> *const c_char;

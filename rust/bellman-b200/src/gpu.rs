@@ -191,6 +191,35 @@ impl Drop for GpuParameters {
     fn drop(&mut self) { unsafe { bb_crs_destroy(self.handle) } }
 }
 
+/// The io::Error `Parameters::read` / `VerifyingKey::read` (groth16/src/lib.rs:158-218, 289-398) return for a status of
+/// bb_params_read / bb_vk_read: InvalidData with the reference's text ("invalid G1", "invalid G2", "point at infinity"),
+/// UnexpectedEof, or Other for a back-end failure (its message)
+fn params_read_error(rc: i32, rep: &bb_params_report) -> io::Error {
+    match rc {
+        BB_ERR_IO_INVALID_DATA => {
+            let g2 = [BB_PARAMS_BETA_G2, BB_PARAMS_GAMMA_G2, BB_PARAMS_DELTA_G2, BB_PARAMS_B_G2].contains(&rep.section);
+            let msg = if rep.why == BB_READ_IDENTITY as i32 { "point at infinity" } else if g2 { "invalid G2" } else { "invalid G1" };
+            io::Error::new(io::ErrorKind::InvalidData, msg)
+        }
+        BB_ERR_IO_UNEXPECTED_EOF => io::Error::new(io::ErrorKind::UnexpectedEof, "failed to fill whole buffer"),
+        _ => io::Error::new(io::ErrorKind::Other, last_error()),
+    }
+}
+
+impl GpuParameters {
+    /// `Parameters::read(bytes, checked)` on the device: the file is decoded and checked there, straight into the resident
+    /// key (bb_params_read), with no `Parameters<Bls12>` on the host.  Same acceptance rules and the same first error as the
+    /// reference.  A caller that also needs the host `VerifyingKey` reads it with `VerifyingKey::read` from the same bytes.
+    pub fn read(worker: &GpuWorker, bytes: &[u8], checked: bool) -> io::Result<GpuParameters> {
+        let (mut handle, mut rep) = (ptr::null_mut(), bb_params_report::default());
+        let rc = unsafe {
+            bb_params_read(worker.ctx, bytes.as_ptr() as _, bytes.len(), 0, checked as i32, &mut handle, ptr::null_mut(), &mut rep)
+        };
+        if rc != BB_OK { return Err(params_read_error(rc, &rep)); }
+        Ok(GpuParameters { ctx: worker.ctx, handle })
+    }
+}
+
 /// What `ProvingAssignment` holds when synthesis is done (groth16/src/prover.rs:57-71,193-215); the fields
 /// are private upstream, so the `b200` feature exposes them to this module (`pub(crate)` in-tree).
 pub struct WitnessView<'a> {
@@ -428,6 +457,16 @@ impl GpuVerifyingKey {
         let mut handle = ptr::null_mut();
         status(unsafe { bb_vk_prepare(worker.ctx, &desc, &mut handle) })?;
         Ok(GpuVerifyingKey { ctx: worker.ctx, handle, ic_len: vk.ic.len() })
+    }
+}
+impl GpuVerifyingKey {
+    /// `VerifyingKey::read(bytes)` + prepare_verifying_key on the device (bb_vk_read), and the bytes it consumed
+    /// (868 + 96 |ic|); a Parameters file starts with its VerifyingKey
+    pub fn read(worker: &GpuWorker, bytes: &[u8]) -> io::Result<(GpuVerifyingKey, usize)> {
+        let (mut handle, mut rep) = (ptr::null_mut(), bb_params_report::default());
+        let rc = unsafe { bb_vk_read(worker.ctx, bytes.as_ptr() as _, bytes.len(), 0, &mut handle, &mut rep) };
+        if rc != BB_OK { return Err(params_read_error(rc, &rep)); }
+        Ok((GpuVerifyingKey { ctx: worker.ctx, handle, ic_len: rep.len[0] }, rep.consumed))
     }
 }
 impl Drop for GpuVerifyingKey {
