@@ -194,6 +194,8 @@ int h_poly_final_device(bb_ctx* ctx, cudaStream_t st, Fr* d_a, const Fr* d_b, co
 int fr_convert_device(bb_ctx* ctx, cudaStream_t st, Fr* d_data, size_t n, bool to_montgomery);
 void ntt_free_tables(bb_ctx* ctx);
 int domain_pointwise_device(bb_ctx* ctx, cudaStream_t st, Fr* d_a, const Fr* d_b, size_t n, int op, const Fr& k);
+// d_out[i] = scale * base^i for i < n (k_powers)
+int powers_device(bb_ctx* ctx, cudaStream_t st, Fr* d_out, size_t n, const Fr& base, const Fr& scale);
 
 // ---- prover.cu ----
 // Queues on `st` the evaluation of a sub-batch's a, b, c into abc (rows a_0 .. a_{B-1}, b_0 .., c_0 .. of m Fr; the first
@@ -207,14 +209,66 @@ int prove_batch_check(const char* fn, const bb_ctx* ctx, const bb_crs* crs, size
 // A single-GPU bb_crs that adopts the five resident vectors h, l, a, b_g1, b_g2 (freed with it); g1 = alpha, beta, delta,
 // g2 = beta, delta (bb_params_read)
 bb_crs* crs_adopt(bb_ctx* ctx, bb_bases* const vec[5], const G1Affine g1[3], const G2Affine g2[2]);
+// What a bb_crs holds (bb_params_write): its context, shard count, the vectors h, l, a, b_g1, b_g2 and g1 = alpha, beta,
+// delta, g2 = beta, delta
+struct CrsView {
+    bb_ctx* ctx;
+    uint32_t shard_count;
+    const bb_bases* vec[5];
+    G1Affine g1[3];
+    G2Affine g2[2];
+};
+CrsView crs_view(const bb_crs* crs);
 
 // ---- verify.cu ----
 // A bb_vk that adopts its device parts (context allocations): alpha_g1, the G2 points in the order delta, gamma, beta, and
 // the resident ic (bb_params_read, bb_vk_read)
 bb_vk* vk_adopt(bb_ctx* ctx, G1Affine* d_alpha, G2Affine* d_g2, bb_bases* ic);
+// The device parts of a bb_vk, as vk_adopt takes them (bb_params_write)
+struct VkView {
+    bb_ctx* ctx;
+    const G1Affine* d_alpha;
+    const G2Affine* d_g2;
+    const bb_bases* ic;
+};
+VkView vk_view(const bb_vk* vk);
+
+// ---- r1cs.cu ----
+// A sparse matrix over Fr as the evaluation kernels read it: row g holds the terms off[g] .. off[g + 1] - 1, each a column
+// index (bit 31 set: coefficient one, the product is skipped) and its coefficient (Montgomery).  rows: the row ids binned
+// by length, n_short rows of at most R1CS_SHORT_MAX terms (one thread each), then n_warp of at most R1CS_WARP_MAX (one
+// warp each), then n_cta longer ones (one CTA each).  Row g of the 3 n goes to out_a[g], out_b[g - n] or out_c[g - 2 n].
+constexpr uint32_t R1CS_ONE_FLAG = 0x80000000u, R1CS_SHORT_MAX = 32, R1CS_WARP_MAX = 2048;
+struct CsrMatrix {
+    const uint32_t* off;
+    const uint32_t* idx;
+    const Fr* coef;
+    const uint32_t* rows;
+    uint32_t n_short, n_warp, n_cta;
+    uint32_t n;                      // rows per output
+};
+// out = M x, with x = input (columns < n_inputs) || aux, queued on `st`
+int csr_eval_queue(bb_ctx* ctx, cudaStream_t st, const CsrMatrix& M, const Fr* input, uint32_t n_inputs, const Fr* aux, Fr* out_a, Fr* out_b,
+                   Fr* out_c);
+// A bb_r1cs as it lies in HBM: the one CSR of its 3 n rows (n constraints incl. the input rows, columns = variables)
+struct R1csView {
+    bb_ctx* ctx;
+    size_t n, n_inputs, n_aux;
+    uint64_t terms;
+    const uint32_t* off;
+    const uint32_t* idx;
+    const Fr* coef;
+};
+R1csView r1cs_view(const bb_r1cs* r1cs);
 
 // ---- capi.cu ----
-int fixed_base_mul_device(bb_ctx* ctx, int group, const Fr* d_scalars, size_t n, bool montgomery, void* d_out, cudaStream_t st);
+// d_table: NULL = the standard generator's cached table, or a table of fixed_table_build
+int fixed_base_mul_device(bb_ctx* ctx, int group, const Fr* d_scalars, size_t n, bool montgomery, void* d_out, cudaStream_t st,
+                          const void* d_table = nullptr);
+// The byte-multiple table of another generator (96 / 192 B affine, not the identity), built on the host and uploaded;
+// the caller zeroes and frees it with fixed_table_free
+int fixed_table_build(int group, const void* gen_affine, void** d_table);
+void fixed_table_free(int group, void* d_table);
 
 // ---- msm.cu ----
 struct MsmResult {

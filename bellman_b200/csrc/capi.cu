@@ -222,10 +222,44 @@ int selftest_run(bb_ctx* ctx, K kernel, const void* a, const void* b, void* o, s
 }  // namespace
 
 namespace bb {
-int fixed_base_mul_device(bb_ctx* ctx, int group, const Fr* d_scalars, size_t n, bool montgomery, void* d_out, cudaStream_t st) {
+int fixed_base_mul_device(bb_ctx* ctx, int group, const Fr* d_scalars, size_t n, bool montgomery, void* d_out, cudaStream_t st,
+                          const void* d_table) {
     if (ctx->device < 0 || ctx->device >= MAX_DEVICES) { set_error("device ordinal out of range"); return BB_ERR_ARG; }
+    if (d_table) {                                        // a caller's table: already built, the generator is not needed
+        if (group == BB_G1) {
+            FixedTable<Fp> t{(G1Affine*)d_table};
+            return fixed_base_mul_dev<Fp>(ctx, t, G1Affine::identity(), d_scalars, n, montgomery, (G1Affine*)d_out, st);
+        }
+        FixedTable<Fp2> t{(G2Affine*)d_table};
+        return fixed_base_mul_dev<Fp2>(ctx, t, G2Affine::identity(), d_scalars, n, montgomery, (G2Affine*)d_out, st);
+    }
     if (group == BB_G1) return fixed_base_mul_dev<Fp>(ctx, g_tab1[ctx->device], g1_generator(), d_scalars, n, montgomery, (G1Affine*)d_out, st);
     return fixed_base_mul_dev<Fp2>(ctx, g_tab2[ctx->device], g2_generator(), d_scalars, n, montgomery, (G2Affine*)d_out, st);
+}
+
+int fixed_table_build(int group, const void* gen, void** d_table) {
+    *d_table = nullptr;
+    if (group == BB_G1) {
+        FixedTable<Fp> t;
+        G1Affine g;
+        std::memcpy(&g, gen, sizeof g);
+        BB_TRY(build_fixed_table(t, g));
+        *d_table = t.d_table;
+    } else {
+        FixedTable<Fp2> t;
+        G2Affine g;
+        std::memcpy(&g, gen, sizeof g);
+        BB_TRY(build_fixed_table(t, g));
+        *d_table = t.d_table;
+    }
+    return BB_OK;
+}
+
+void fixed_table_free(int group, void* d_table) {
+    if (!d_table) return;
+    cudaMemsetAsync(d_table, 0, (size_t)32 * 255 * (group == BB_G1 ? sizeof(G1Affine) : sizeof(G2Affine)));
+    cudaDeviceSynchronize();
+    cudaFree(d_table);
 }
 }  // namespace bb
 

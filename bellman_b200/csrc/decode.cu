@@ -322,6 +322,36 @@ __global__ void __launch_bounds__(DECODE_THREADS) k_params_decode_g2(const uint8
     else out[i] = p;
 }
 
+// ---- Parameters::write (lib.rs:258-287): to_uncompressed, the inverse of the decoders above -----------------------------
+// canonical big-endian coordinates (G2: x.c1 | x.c0 | y.c1 | y.c0); the identity is the infinity flag 0x40, then zeros
+BB_D void g1_store_uncompressed(const G1Affine& p, uint8_t* o) {
+    if (p.is_identity()) { o[0] = 0x40; for (int k = 1; k < 96; k++) o[k] = 0; return; }
+    fp_store_be(fp_to_canonical(p.x), o);
+    fp_store_be(fp_to_canonical(p.y), o + 48);
+}
+BB_D void g2_store_uncompressed(const G2Affine& p, uint8_t* o) {
+    if (p.is_identity()) { o[0] = 0x40; for (int k = 1; k < 192; k++) o[k] = 0; return; }
+    fp_store_be(fp_to_canonical(p.x.c1), o);
+    fp_store_be(fp_to_canonical(p.x.c0), o + 48);
+    fp_store_be(fp_to_canonical(p.y.c1), o + 96);
+    fp_store_be(fp_to_canonical(p.y.c0), o + 144);
+}
+// n points -> out[0 .. 96 n) (G2: 192 n), one thread per point; prefix != 0: thread 0 also writes n as the big-endian u32 in
+// the four bytes before out (launched with at least one thread)
+BB_D void store_prefix(uint8_t* o, size_t n) {
+    o[0] = (uint8_t)(n >> 24); o[1] = (uint8_t)(n >> 16); o[2] = (uint8_t)(n >> 8); o[3] = (uint8_t)n;
+}
+__global__ void __launch_bounds__(128) k_params_encode_g1(const G1Affine* __restrict__ pts, size_t n, int prefix, uint8_t* out) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (prefix && i == 0) store_prefix(out - 4, n);
+    if (i < n) g1_store_uncompressed(pts[i], out + i * 96);
+}
+__global__ void __launch_bounds__(128) k_params_encode_g2(const G2Affine* __restrict__ pts, size_t n, int prefix, uint8_t* out) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (prefix && i == 0) store_prefix(out - 4, n);
+    if (i < n) g2_store_uncompressed(pts[i], out + i * 192);
+}
+
 constexpr int PARAMS_SECTIONS = 12, VK_SECTIONS = 7;
 const char* const kSection[PARAMS_SECTIONS] = {"alpha_g1", "beta_g1", "beta_g2", "gamma_g2", "delta_g1", "delta_g2",
                                                "ic", "h", "l", "a", "b_g1", "b_g2"};
@@ -694,6 +724,77 @@ int bb_params_read(bb_ctx* ctx, const void* bytes, size_t len, int on_device, in
 
 int bb_vk_read(bb_ctx* ctx, const void* bytes, size_t len, int on_device, bb_vk** vk_out, bb_params_report* report) {
     return params_read_impl(ctx, bytes, len, on_device, 1, VK_SECTIONS, nullptr, vk_out, report);
+}
+
+int bb_params_write(bb_ctx* ctx, const bb_crs* crs, const bb_vk* vk, int vk_only, void* out, size_t cap, int out_on_device, size_t* len_out) {
+    if (!ctx || !crs || !vk || !len_out) { set_error("bb_params_write: null argument"); return BB_ERR_ARG; }
+    const CrsView K = crs_view(crs);
+    const VkView V = vk_view(vk);
+    if (K.ctx != ctx || V.ctx != ctx) { set_error("bb_params_write: the key lives on another context"); return BB_ERR_ARG; }
+    if (K.shard_count > 1) { set_error("bb_params_write: shard %u of a sharded key: only a whole key can be written", K.shard_count); return BB_ERR_ARG; }
+    const size_t n_ic = V.ic->n;
+    size_t len = 868 + 96 * n_ic;
+    if (!vk_only) len += 5 * 4 + 96 * (K.vec[0]->n + K.vec[1]->n + K.vec[2]->n + K.vec[3]->n) + 192 * K.vec[4]->n;
+    BB_CUDA(cudaSetDevice(ctx->device));
+    G1Affine v_alpha;
+    G2Affine v_g2[3];                                             // delta, gamma, beta
+    BB_CUDA(cudaMemcpy(&v_alpha, V.d_alpha, sizeof v_alpha, cudaMemcpyDeviceToHost));
+    BB_CUDA(cudaMemcpy(v_g2, V.d_g2, sizeof v_g2, cudaMemcpyDeviceToHost));
+    if (std::memcmp(&v_alpha, &K.g1[0], sizeof v_alpha) || std::memcmp(&v_g2[2], &K.g2[0], sizeof(G2Affine)) ||
+        std::memcmp(&v_g2[0], &K.g2[1], sizeof(G2Affine))) {
+        set_error("bb_params_write: not this key's verifying key (alpha_g1, beta_g2 or delta_g2 differ)");
+        return BB_ERR_ARG;
+    }
+    *len_out = len;
+    if (!out) return BB_OK;
+    if (cap < len) { set_error("bb_params_write: %zu bytes of room for a %zu-byte key", cap, len); return BB_ERR_ARG; }
+    NvtxRange nvtx("params_write");
+    cudaStream_t st = ctx->main_stream;
+    StageTimer tm(ctx, st);
+    tm.mark("params.begin");
+    DevBuf d_out, d_g1x;
+    uint8_t* o = (uint8_t*)out;
+    if (!out_on_device) {
+        BB_TRY(d_out.alloc(ctx, len));
+        o = d_out.as<uint8_t>();
+    }
+    const G1Affine g1x[2] = {K.g1[1], K.g1[2]};                  // beta_g1, delta_g1: only the crs holds them
+    BB_TRY(d_g1x.alloc(ctx, sizeof g1x));
+    BB_CUDA(cudaMemcpyAsync(d_g1x.p, g1x, sizeof g1x, cudaMemcpyHostToDevice, st));
+    size_t off = 0;
+    auto g1 = [&](const void* pts, size_t n, bool prefix) {
+        if (prefix) off += 4;
+        k_params_encode_g1<<<cdiv(n ? n : 1, 128), 128, 0, st>>>((const G1Affine*)pts, n, prefix ? 1 : 0, o + off);
+        ctx->count_launch();
+        off += 96 * n;
+    };
+    auto g2 = [&](const void* pts, size_t n, bool prefix) {
+        if (prefix) off += 4;
+        k_params_encode_g2<<<cdiv(n ? n : 1, 128), 128, 0, st>>>((const G2Affine*)pts, n, prefix ? 1 : 0, o + off);
+        ctx->count_launch();
+        off += 192 * n;
+    };
+    g1(V.d_alpha, 1, false);                                      // VerifyingKey::write (lib.rs:143-156)
+    g1(d_g1x.as<G1Affine>(), 1, false);
+    g2(V.d_g2 + 2, 1, false);
+    g2(V.d_g2 + 1, 1, false);
+    g1(d_g1x.as<G1Affine>() + 1, 1, false);
+    g2(V.d_g2, 1, false);
+    g1(V.ic->d_points, n_ic, true);
+    if (!vk_only) {                                               // then h, l, a, b_g1, b_g2 (lib.rs:258-287)
+        for (int k = 0; k < 4; k++) g1(K.vec[k]->d_points, K.vec[k]->n, true);
+        g2(K.vec[4]->d_points, K.vec[4]->n, true);
+    }
+    BB_CUDA(cudaGetLastError());
+    tm.mark("params.encode");
+    if (!out_on_device) {
+        BB_CUDA(cudaMemcpyAsync(out, o, len, cudaMemcpyDeviceToHost, st));
+        ctx->d2h_bytes += len;
+    }
+    tm.mark("params.download");
+    BB_CUDA(cudaStreamSynchronize(st));
+    tm.report(len);
+    return BB_OK;
 }
 
 }  // extern "C"

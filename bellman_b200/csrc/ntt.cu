@@ -500,6 +500,15 @@ int domain_pointwise_device(bb_ctx* ctx, cudaStream_t st, Fr* d_a, const Fr* d_b
     return BB_OK;
 }
 
+int powers_device(bb_ctx* ctx, cudaStream_t st, Fr* d_out, size_t n, const Fr& base, const Fr& scale) {
+    if (!n) return BB_OK;
+    const size_t threads = (n + 31) / 32;
+    k_powers<<<cdiv(threads, 256), 256, 0, st>>>(d_out, n, base, scale);
+    ctx->count_launch();
+    BB_CUDA(cudaGetLastError());
+    return BB_OK;
+}
+
 void ntt_free_tables(bb_ctx* ctx) {
     for (auto& kv : ctx->ntt_tables) {
         NttTables* t = kv.second;

@@ -228,6 +228,10 @@ bb_crs* crs_adopt(bb_ctx* ctx, bb_bases* const vec[5], const G1Affine g1[3], con
     crs->beta_g2 = g2[0]; crs->delta_g2 = g2[1];
     return crs;
 }
+CrsView crs_view(const bb_crs* crs) {
+    return CrsView{crs->ctx, crs->shard_count, {crs->h, crs->l, crs->a, crs->b_g1, crs->b_g2}, {crs->alpha_g1, crs->beta_g1, crs->delta_g1},
+                   {crs->beta_g2, crs->delta_g2}};
+}
 }  // namespace bb
 
 namespace {

@@ -24,9 +24,9 @@ using namespace bb;
 
 namespace {
 
-constexpr uint32_t ONE_FLAG = 0x80000000u;
-constexpr uint32_t SHORT_MAX = 32;     // terms: one thread per row up to here
-constexpr uint32_t WARP_MAX = 2048;    // one warp per row up to here, one CTA above
+constexpr uint32_t ONE_FLAG = R1CS_ONE_FLAG;
+constexpr uint32_t SHORT_MAX = R1CS_SHORT_MAX;   // terms: one thread per row up to here
+constexpr uint32_t WARP_MAX = R1CS_WARP_MAX;     // one warp per row up to here, one CTA above
 constexpr int GROUP_THREADS = 256;
 
 struct EvalArgs {
@@ -133,23 +133,38 @@ int stage_witness(bb_ctx* ctx, cudaStream_t st, const void* input, size_t n_inpu
 
 // queues the evaluation of all 3 N rows on `st`
 int r1cs_eval_queue(bb_ctx* ctx, cudaStream_t st, const bb_r1cs* R, const Fr* d_in, const Fr* d_aux, Fr* oa, Fr* ob, Fr* oc) {
-    EvalArgs A{(const uint32_t*)R->d_off, (const uint32_t*)R->d_idx, (const Fr*)R->d_coef, d_in, d_aux, oa, ob, oc,
-               (uint32_t)R->n_inputs, (uint32_t)R->n};
-    const uint32_t* rows = (const uint32_t*)R->d_rows;
-    if (R->n_short) { k_r1cs_rows_thread<<<cdiv(R->n_short, 128), 128, 0, st>>>(A, rows, R->n_short); ctx->count_launch(); }
-    if (R->n_warp) {
-        k_r1cs_rows_group<32><<<cdiv(R->n_warp, GROUP_THREADS / 32), GROUP_THREADS, 0, st>>>(A, rows + R->n_short, R->n_warp);
+    const CsrMatrix M{(const uint32_t*)R->d_off, (const uint32_t*)R->d_idx, (const Fr*)R->d_coef, (const uint32_t*)R->d_rows,
+                      R->n_short, R->n_warp, R->n_cta, (uint32_t)R->n};
+    return csr_eval_queue(ctx, st, M, d_in, (uint32_t)R->n_inputs, d_aux, oa, ob, oc);
+}
+
+}  // namespace
+
+namespace bb {
+
+int csr_eval_queue(bb_ctx* ctx, cudaStream_t st, const CsrMatrix& M, const Fr* input, uint32_t n_inputs, const Fr* aux, Fr* oa, Fr* ob,
+                   Fr* oc) {
+    EvalArgs A{M.off, M.idx, M.coef, input, aux, oa, ob, oc, n_inputs, M.n};
+    const uint32_t* rows = M.rows;
+    if (M.n_short) { k_r1cs_rows_thread<<<cdiv(M.n_short, 128), 128, 0, st>>>(A, rows, M.n_short); ctx->count_launch(); }
+    if (M.n_warp) {
+        k_r1cs_rows_group<32><<<cdiv(M.n_warp, GROUP_THREADS / 32), GROUP_THREADS, 0, st>>>(A, rows + M.n_short, M.n_warp);
         ctx->count_launch();
     }
-    if (R->n_cta) {
-        k_r1cs_rows_group<GROUP_THREADS><<<R->n_cta, GROUP_THREADS, 0, st>>>(A, rows + R->n_short + R->n_warp, R->n_cta);
+    if (M.n_cta) {
+        k_r1cs_rows_group<GROUP_THREADS><<<M.n_cta, GROUP_THREADS, 0, st>>>(A, rows + M.n_short + M.n_warp, M.n_cta);
         ctx->count_launch();
     }
     BB_CUDA(cudaGetLastError());
     return BB_OK;
 }
 
-}  // namespace
+R1csView r1cs_view(const bb_r1cs* R) {
+    return R1csView{R->ctx, R->n, R->n_inputs, R->n_aux, R->nnz[0] + R->nnz[1] + R->nnz[2], (const uint32_t*)R->d_off,
+                    (const uint32_t*)R->d_idx, (const Fr*)R->d_coef};
+}
+
+}  // namespace bb
 
 extern "C" {
 

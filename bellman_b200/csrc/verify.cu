@@ -624,6 +624,7 @@ bb_vk* vk_adopt(bb_ctx* ctx, G1Affine* d_alpha, G2Affine* d_g2, bb_bases* ic) {
     vk->ic_len = ic->n;
     return vk;
 }
+VkView vk_view(const bb_vk* vk) { return VkView{vk->ctx, vk->d_alpha, vk->d_g2, vk->ic}; }
 }  // namespace bb
 
 extern "C" {

@@ -18,9 +18,12 @@ The result maps the names of groth16::Parameters (vk_g1 = alpha, beta, delta; vk
 delta; ic, h, l, a, b_g1, b_g2) to Montgomery-limb arrays, the layout `Parameters(worker, p)` and
 `params_io.write_parameters` take.
 """
+import ctypes as C
+
 import numpy as np
 
-from . import (EvaluationDomain, G1, G2, FORM_CANONICAL, SynthesisError, UnexpectedIdentity, fixed_base_mul)
+from . import (EvaluationDomain, G1, G2, FORM_CANONICAL, SynthesisError, UnexpectedIdentity, _c64, _check, _ERRORS, fixed_base_mul,
+               load_library)
 
 FR_MODULUS = EvaluationDomain.FR_MODULUS
 _R = 1 << 256
@@ -28,7 +31,16 @@ _R_INV = pow(_R, -1, FR_MODULUS)
 
 
 class UnconstrainedVariable(SynthesisError):
-    """SynthesisError::UnconstrainedVariable (generator.rs:466-470)"""
+    """SynthesisError::UnconstrainedVariable (generator.rs:466-470).  From the device generator: `index`, the first aux
+    variable whose l element is the identity."""
+
+    def __init__(self, message, index=None):
+        super().__init__(message)
+        self.index = index
+
+
+BB_ERR_UNCONSTRAINED_VARIABLE = 4
+_ERRORS[BB_ERR_UNCONSTRAINED_VARIABLE] = UnconstrainedVariable
 
 
 class KeypairAssembly:
@@ -126,3 +138,62 @@ def generate_parameters(worker, assembly, alpha, beta, gamma, delta, tau, g1_sca
         vk_g1=g1_mul([alpha, beta, delta]), vk_g2=g2_mul([beta, gamma, delta]),
         ic=g1_mul(ic_k), h=h, l=g1_mul(l_k), a=g1_mul(a_k), b_g1=g1_mul(b_k), b_g2=g2_mul(b_k),
         num_inputs=asm.num_inputs, num_aux=asm.num_aux, m=m)
+
+
+# --------------------------------------------------------------------------------------------
+# the whole generator on the device (bb_groth16_generate, csrc/generate.cu)
+# --------------------------------------------------------------------------------------------
+class _Toxic(C.Structure):
+    """bb_toxic"""
+    _fields_ = [("g1", C.c_void_p), ("g2", C.c_void_p), ("alpha", C.c_uint8 * 32), ("beta", C.c_uint8 * 32), ("gamma", C.c_uint8 * 32),
+                ("delta", C.c_uint8 * 32), ("tau", C.c_uint8 * 32)]
+
+
+class GenerateReport(C.Structure):
+    """bb_generate_report"""
+    _fields_ = [("len", C.c_size_t * 6), ("m", C.c_size_t), ("unconstrained", C.c_size_t)]
+
+
+def _device_generate(worker, r1cs, toxic):
+    from . import Parameters
+    from .verifier import PreparedVerifyingKey
+    crs, vk, rep = C.c_void_p(), C.c_void_p(), GenerateReport()
+    rc = load_library().bb_groth16_generate(worker._h, r1cs._h, C.byref(toxic) if toxic is not None else None, C.byref(crs), C.byref(vk),
+                                            C.byref(rep))
+    if rc == BB_ERR_UNCONSTRAINED_VARIABLE:
+        raise UnconstrainedVariable(load_library().bb_last_error().decode(errors="replace"), index=int(rep.unconstrained))
+    _check(rc)
+    lens = dict(zip(("ic", "h", "l", "a", "b_g1", "b_g2"), (int(v) for v in rep.len)))
+    return Parameters._from_handle(worker, crs, lens), PreparedVerifyingKey._from_handle(worker, vk, lens["ic"])
+
+
+def generate_parameters_device(worker, r1cs, alpha, beta, gamma, delta, tau, g1=None, g2=None):
+    """generate_parameters (generator.rs:159-507) for the constraint system resident in `r1cs` (an R1CS of this worker),
+    computed on the device -> (Parameters, PreparedVerifyingKey).  alpha..tau: integers in [0, r).  g1, g2: the generators
+    as affine points in the library's format ((12,) / (24,) uint64 Montgomery), None = the standard ones.  The same points
+    generate_parameters gives for the KeypairAssembly the constraint system was built from (with g1_scalar, g2_scalar:
+    g1 = [g1_scalar] G1).  Raises UnexpectedIdentity (gamma or delta zero), UnconstrainedVariable (with .index) or
+    BackendError for bad arguments."""
+    t = _Toxic()
+    keep = []
+    for name, g, width in (("g1", g1, 12), ("g2", g2, 24)):
+        if g is not None:
+            arr = _c64(g, width).copy()
+            keep.append(arr)
+            setattr(t, name, arr.ctypes.data)
+    for name, v in (("alpha", alpha), ("beta", beta), ("gamma", gamma), ("delta", delta), ("tau", tau)):
+        v = int(v)
+        if not 0 <= v < 1 << 256:
+            raise ValueError(f"{name} is not a 256-bit integer")
+        getattr(t, name)[:] = v.to_bytes(32, "little")
+    try:
+        return _device_generate(worker, r1cs, t)
+    finally:
+        C.memset(C.addressof(t), 0, C.sizeof(t))
+        del keep
+
+
+def generate_random_parameters_device(worker, r1cs):
+    """generate_random_parameters (generator.rs:21-40) on the device: the toxic waste and the generators are drawn by the
+    library from the operating system and never leave it -> (Parameters, PreparedVerifyingKey)"""
+    return _device_generate(worker, r1cs, None)

@@ -264,3 +264,23 @@ def write_parameters(p):
         out += struct.pack(">I", arr.shape[0])
         out += _abi_to_coords(arr, 4 if g2 else 2, g2).tobytes()
     return bytes(out)
+
+
+def write_parameters_device(params, pvk, verifying_key_only=False, out=None):
+    """Parameters::write (or with verifying_key_only=True VerifyingKey::write) of a resident key, encoded on the device
+    (bb_params_write): byte for byte write_parameters of the same points.  params: a single-GPU Parameters; pvk: its
+    PreparedVerifyingKey (it holds gamma_g2 and ic).  Returns the bytes; or with out = (device_ptr, capacity) writes them
+    there and returns their length.  A sharded key, a verifying key of another key or too small a buffer raise
+    BackendError."""
+    lib = load_library()
+    n = C.c_size_t()
+    _check(lib.bb_params_write(params.worker._h, params._h, pvk._h, C.c_int(1 if verifying_key_only else 0), None, C.c_size_t(0),
+                               C.c_int(0), C.byref(n)))
+    if out is not None:
+        _check(lib.bb_params_write(params.worker._h, params._h, pvk._h, C.c_int(1 if verifying_key_only else 0), C.c_void_p(_addr(out[0])),
+                                   C.c_size_t(int(out[1])), C.c_int(1), C.byref(n)))
+        return int(n.value)
+    buf = np.empty(n.value, np.uint8)
+    _check(lib.bb_params_write(params.worker._h, params._h, pvk._h, C.c_int(1 if verifying_key_only else 0), buf.ctypes.data_as(C.c_void_p),
+                               C.c_size_t(buf.size), C.c_int(0), C.byref(n)))
+    return buf.tobytes()

@@ -39,6 +39,7 @@ typedef enum bb_status {
     BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE = 1, /* domain.rs:57-59 */
     BB_ERR_UNEXPECTED_IDENTITY = 2,         /* multiexp.rs:63-65, prover.rs:320-324 */
     BB_ERR_IO_UNEXPECTED_EOF = 3,           /* multiexp.rs:55-61,74-80 */
+    BB_ERR_UNCONSTRAINED_VARIABLE = 4,      /* generator.rs:464-470 */
     BB_ERR_DENSITY_MISMATCH = 5,            /* the assert! at multiexp.rs:324-329 (a panic upstream) */
     /* VerificationError (src/lib.rs:353-358) */
     BB_ERR_INVALID_VERIFYING_KEY = 6,       /* inputs.len() + 1 != ic.len(): verifier.rs:28-30, batch.rs:105-111 */
@@ -63,6 +64,7 @@ typedef struct bb_bases bb_bases;     /* device-resident Arc<Vec<G::Affine>> (gr
 typedef struct bb_msm_job bb_msm_job; /* Waiter<Result<G, SynthesisError>> (src/multicore.rs:94-118) */
 typedef struct bb_crs bb_crs;         /* device-resident groth16::Parameters (groth16/src/lib.rs:222-244) */
 typedef struct bb_prove bb_prove;     /* one create_proof in flight between bb_groth16_prove_begin and _end */
+typedef struct bb_vk bb_vk;           /* device-resident PreparedVerifyingKey (groth16/src/lib.rs:400-409), see bb_vk_prepare */
 
 const char* bb_last_error(void);
 int bb_version(void);
@@ -89,8 +91,8 @@ void bb_ctx_destroy(bb_ctx* ctx);
  *   params_read_chunk  bb_params_read / bb_vk_read from host memory: staging bytes per chunk (default 64 MiB; rounded
  *                      down to whole points, at least one point)
  *   ntt_radix8         1 = register radix-8 NTT windows (default 0: measured slower), ntt_tile_log, ntt_col_bits
- *   profile            1 = CUDA-event timing of the MSM stages, and of the verify.*, decode.*, r1cs.* and params.* stages
- *                      (bb_profile_read) */
+ *   profile            1 = CUDA-event timing of the MSM stages, and of the verify.*, decode.*, r1cs.*, params.* and
+ *                      generate.* stages (bb_profile_read) */
 int bb_ctx_set_option(bb_ctx* ctx, const char* key, long value);
 int bb_ctx_synchronize(bb_ctx* ctx);
 /* counters for the harness: number of kernels this context has launched */
@@ -339,6 +341,41 @@ int bb_groth16_prove_r1cs_batch(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* r
                                 const void* aux, size_t n_aux, size_t count, int on_device, const uint8_t* r, const uint8_t* s,
                                 uint8_t* proofs, int* status);
 
+/* ---- generating keys: generate_parameters / generate_random_parameters (groth16/src/generator.rs:21-40,159-507) ----------
+ * The key of a resident constraint system, computed on the device, element for element the reference's: the rows are the
+ * bb_r1cs rows including its input rows (generator.rs:193-202), m = the next power of two >= rows; h[i] = [tau^i t(tau) /
+ * delta] g1 for i < m - 1 with t(tau) = tau^m - 1; L = ifft of the m powers of tau; per variable j at_j, bt_j, ct_j = the sums
+ * of coeff * L_row over its terms in A, B, C; ic (inputs, inv = 1/gamma) and l (aux, inv = 1/delta) = [(beta at + alpha bt +
+ * ct) inv] g1; a, b_g1, b_g2 = [at] g1, [bt] g1, [bt] g2 with the zero scalars dropped in variable order (the evaluated
+ * scalar decides, not the prover's density: cancelling terms give a dropped element); the verifying key [alpha] g1,
+ * [beta] g1, [delta] g1, [beta] g2, [gamma] g2, [delta] g2.
+ * Errors, in this order, all before any device work but the last:
+ *   BB_ERR_ARG                     NULL ctx, r1cs or crs_out; an r1cs of another context; a scalar >= r; g1 or g2 the
+ *                                  identity, off the curve or outside the subgroup (the reference's types cannot hold such
+ *                                  a point; with non-identity generators "scalar zero" and "point is the identity" agree)
+ *   BB_ERR_UNEXPECTED_IDENTITY     gamma = 0, then delta = 0 (generator.rs:228-243)
+ *   BB_ERR_UNCONSTRAINED_VARIABLE  an l scalar is zero (found after the evaluation); report->unconstrained and
+ *                                  bb_last_error() name the first such aux index
+ * alpha = 0, beta = 0, tau = 0 and tau a root of unity of the domain (every h element the identity) are accepted.  On
+ * failure *crs_out and *vk_out are NULL and every block is back in the context's cache.  The key is a single-GPU key
+ * (shard 0 of 1).  toxic == NULL: generate_random_parameters -- alpha, beta, gamma, delta, tau and the two generators (as
+ * random multiples of the standard ones) drawn with getrandom, zeros redrawn; none of them leaves the call.
+ * Toxic waste: every device block that held a scalar derived from it (powers of tau, Lagrange coefficients, QAP values,
+ * compacted scalars) is zeroed before it returns to the context's cache, and the host copies are wiped.  The fixed-base
+ * multiplications run in variable time, as the reference's wNAF does. */
+typedef struct bb_toxic {
+    const void* g1; const void* g2;    /* 96 / 192 B affine in the format above; NULL = the standard generator */
+    uint8_t alpha[32], beta[32], gamma[32], delta[32], tau[32];   /* canonical little-endian, < r */
+} bb_toxic;
+typedef struct bb_generate_report {
+    size_t len[6];          /* ic, h, l, a, b_g1, b_g2 */
+    size_t m;               /* the domain size */
+    size_t unconstrained;   /* BB_ERR_UNCONSTRAINED_VARIABLE: the first aux index whose l scalar is zero (SIZE_MAX if none) */
+} bb_generate_report;
+/* vk_out (the PreparedVerifyingKey) and report may be NULL */
+int bb_groth16_generate(bb_ctx* ctx, const bb_r1cs* r1cs, const bb_toxic* toxic, bb_crs** crs_out, bb_vk** vk_out,
+                        bb_generate_report* report);
+
 /* ---- verification: groth16/src/verifier.rs and groth16/src/verifier/batch.rs ------------------
  * Points are taken as valid curve and subgroup elements, as the reference's Proof / VerifyingKey types guarantee
  * through read(); bb_points_validate applies those checks.  The identity is allowed anywhere: a pair with an identity
@@ -349,7 +386,6 @@ typedef struct bb_vk_desc {
     const void* beta_g2; const void* gamma_g2; const void* delta_g2;  /* 192 B each */
     const void* ic; size_t ic_len;                                    /* 96 B each */
 } bb_vk_desc;
-typedef struct bb_vk bb_vk;
 int bb_vk_prepare(bb_ctx* ctx, const bb_vk_desc* desc, bb_vk** out);
 void bb_vk_destroy(bb_vk* vk);
 
@@ -448,6 +484,15 @@ int bb_params_read(bb_ctx* ctx, const void* bytes, size_t len, int on_device, in
                    bb_crs** crs_out, bb_vk** vk_out, bb_params_report* report);
 /* VerifyingKey::read + prepare_verifying_key: the first 868 + 96 |ic| bytes of a VerifyingKey or Parameters file */
 int bb_vk_read(bb_ctx* ctx, const void* bytes, size_t len, int on_device, bb_vk** vk_out, bb_params_report* report);
+/* Parameters::write / VerifyingKey::write (groth16/src/lib.rs:258-287, 143-156) of a resident key: byte for byte the format
+ * bb_params_read reads (canonical big-endian coordinates, G2 as x.c1 | x.c0 | y.c1 | y.c0, the identity as 0x40 then
+ * zeros), encoded on the device.  vk holds gamma_g2 and ic, crs the rest (beta_g1 and delta_g1 live only there, so crs is
+ * required with vk_only too).  vk_only: the VerifyingKey alone, the first 868 + 96 |ic| bytes.  out: host memory, or
+ * device memory with out_on_device != 0; out == NULL only sets *len_out.  BB_ERR_ARG, before any device work: NULL ctx,
+ * crs, vk or len_out; a key of another context; a sharded crs; a vk whose alpha_g1, beta_g2 and delta_g2 are not the
+ * crs's ("not this key's verifying key"); cap < the length (with *len_out = the length needed). */
+int bb_params_write(bb_ctx* ctx, const bb_crs* crs, const bb_vk* vk, int vk_only, void* out, size_t cap, int out_on_device,
+                    size_t* len_out);
 
 /* ---- tuning per key ------------------------------------------------------------------------
  * The MSM has several forms with identical results (per-window bucket sets; one bucket set over resident window

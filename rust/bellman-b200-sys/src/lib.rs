@@ -18,6 +18,7 @@ pub const BB_OK: c_int = 0;
 pub const BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE: c_int = 1;
 pub const BB_ERR_UNEXPECTED_IDENTITY: c_int = 2;
 pub const BB_ERR_IO_UNEXPECTED_EOF: c_int = 3;
+pub const BB_ERR_UNCONSTRAINED_VARIABLE: c_int = 4;
 pub const BB_ERR_DENSITY_MISMATCH: c_int = 5;
 pub const BB_ERR_INVALID_VERIFYING_KEY: c_int = 6;
 pub const BB_ERR_INVALID_PROOF: c_int = 7;
@@ -123,6 +124,19 @@ pub struct bb_params_report {
     pub len: [usize; 6], pub consumed: usize, pub section: c_int, pub index: usize, pub why: c_int,
 }
 
+// generate_parameters on the device: the toxic waste (canonical little-endian scalars; NULL generators = the standard ones)
+#[repr(C)]
+pub struct bb_toxic {
+    pub g1: *const c_void, pub g2: *const c_void,
+    pub alpha: [u8; 32], pub beta: [u8; 32], pub gamma: [u8; 32], pub delta: [u8; 32], pub tau: [u8; 32],
+}
+
+#[repr(C)]
+#[derive(Default)]
+pub struct bb_generate_report {
+    pub len: [usize; 6], pub m: usize, pub unconstrained: usize,
+}
+
 extern "C" {
     pub fn bb_last_error() -> *const c_char;
     pub fn bb_version() -> c_int;
@@ -218,6 +232,10 @@ extern "C" {
                           crs_out: *mut *mut bb_crs, vk_out: *mut *mut bb_vk, report: *mut bb_params_report) -> c_int;
     pub fn bb_vk_read(ctx: *mut bb_ctx, bytes: *const c_void, len: usize, on_device: c_int, vk_out: *mut *mut bb_vk,
                       report: *mut bb_params_report) -> c_int;
+    pub fn bb_params_write(ctx: *mut bb_ctx, crs: *const bb_crs, vk: *const bb_vk, vk_only: c_int, out: *mut c_void, cap: usize,
+                           out_on_device: c_int, len_out: *mut usize) -> c_int;
+    pub fn bb_groth16_generate(ctx: *mut bb_ctx, r1cs: *const bb_r1cs, toxic: *const bb_toxic, crs_out: *mut *mut bb_crs,
+                               vk_out: *mut *mut bb_vk, report: *mut bb_generate_report) -> c_int;
 
     pub fn bb_tuning_count() -> c_int;
     pub fn bb_tuning_name(index: c_int) -> *const c_char;

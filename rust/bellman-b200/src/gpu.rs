@@ -27,6 +27,7 @@ fn status(rc: i32) -> Result<(), SynthesisError> {
         BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE => Err(SynthesisError::PolynomialDegreeTooLarge),
         BB_ERR_UNEXPECTED_IDENTITY => Err(SynthesisError::UnexpectedIdentity),
         BB_ERR_IO_UNEXPECTED_EOF => Err(io::Error::new(io::ErrorKind::UnexpectedEof, "expected more bases from source").into()),
+        BB_ERR_UNCONSTRAINED_VARIABLE => Err(SynthesisError::UnconstrainedVariable),
         BB_ERR_DENSITY_MISMATCH => panic!("assertion failed: query_size == exponents.len()"), // the assert! of multiexp.rs:324-329
         _ => Err(io::Error::new(io::ErrorKind::Other, last_error()).into()),
     }
@@ -689,3 +690,56 @@ pub fn verify_each_bytes_b200(worker: &GpuWorker, pvk: &GpuVerifyingKey, items: 
 
 #[allow(dead_code)]
 fn _projective_types_are_what_wait_returns(_: G1Projective, _: G2Projective) {}
+
+impl GpuParameters {
+    /// `generate_parameters(circuit, g1, g2, alpha, beta, gamma, delta, tau)` (groth16/src/generator.rs:159-507) for the
+    /// circuit whose constraint system `r1cs` holds, computed on the device (bb_groth16_generate): the same points, element
+    /// for element, as a resident key and its prepared verifying key.  Nothing but the toxic waste crosses the bus; the
+    /// library wipes its copies of it.  Errors as the reference: UnexpectedIdentity for gamma or delta zero,
+    /// UnconstrainedVariable.
+    #[allow(clippy::too_many_arguments)]
+    pub fn generate(worker: &GpuWorker, r1cs: &GpuR1cs, g1: G1Projective, g2: G2Projective, alpha: Scalar, beta: Scalar, gamma: Scalar,
+                    delta: Scalar, tau: Scalar) -> Result<(GpuParameters, GpuVerifyingKey), SynthesisError> {
+        let (mut p1, mut p2) = (vec![0u64; G1Affine::WORDS], vec![0u64; G2Affine::WORDS]);
+        g1.to_affine().to_b200(&mut p1);
+        g2.to_affine().to_b200(&mut p2);
+        let mut toxic = bb_toxic {
+            g1: p1.as_ptr() as _, g2: p2.as_ptr() as _, alpha: alpha.to_repr(), beta: beta.to_repr(), gamma: gamma.to_repr(),
+            delta: delta.to_repr(), tau: tau.to_repr(),
+        };
+        let res = generate_impl(worker, r1cs, &toxic);
+        for k in [&mut toxic.alpha, &mut toxic.beta, &mut toxic.gamma, &mut toxic.delta, &mut toxic.tau] {
+            for b in k.iter_mut() { unsafe { ptr::write_volatile(b, 0) } }
+        }
+        res
+    }
+
+    /// `Parameters::write` (groth16/src/lib.rs:258-287) of this resident key, encoded on the device (bb_params_write): the
+    /// bytes the reference writes for the same key.  `vk` is this key's prepared verifying key (it holds gamma_g2 and ic).
+    pub fn write<W: io::Write>(&self, vk: &GpuVerifyingKey, writer: W) -> io::Result<()> { self.write_impl(vk, false, writer) }
+
+    /// `VerifyingKey::write` (groth16/src/lib.rs:143-156) of this key's verifying key
+    pub fn write_verifying_key<W: io::Write>(&self, vk: &GpuVerifyingKey, writer: W) -> io::Result<()> { self.write_impl(vk, true, writer) }
+
+    fn write_impl<W: io::Write>(&self, vk: &GpuVerifyingKey, vk_only: bool, mut writer: W) -> io::Result<()> {
+        let mut len = 0usize;
+        let rc = unsafe { bb_params_write(self.ctx, self.handle, vk.handle, vk_only as i32, ptr::null_mut(), 0, 0, &mut len) };
+        if rc != BB_OK { return Err(io::Error::new(io::ErrorKind::Other, last_error())); }
+        let mut buf = vec![0u8; len];
+        let rc = unsafe { bb_params_write(self.ctx, self.handle, vk.handle, vk_only as i32, buf.as_mut_ptr() as _, len, 0, &mut len) };
+        if rc != BB_OK { return Err(io::Error::new(io::ErrorKind::Other, last_error())); }
+        writer.write_all(&buf)
+    }
+}
+
+fn generate_impl(worker: &GpuWorker, r1cs: &GpuR1cs, toxic: *const bb_toxic) -> Result<(GpuParameters, GpuVerifyingKey), SynthesisError> {
+    let (mut crs, mut vk, mut rep) = (ptr::null_mut(), ptr::null_mut(), bb_generate_report::default());
+    status(unsafe { bb_groth16_generate(worker.ctx, r1cs.handle, toxic, &mut crs, &mut vk, &mut rep) })?;
+    Ok((GpuParameters { ctx: worker.ctx, handle: crs }, GpuVerifyingKey { ctx: worker.ctx, handle: vk, ic_len: rep.len[0] }))
+}
+
+/// `generate_random_parameters` (groth16/src/generator.rs:21-40) on the device: the library draws the toxic waste and the
+/// generators from the operating system (getrandom), and none of them leaves it.
+pub fn generate_random_parameters_b200(worker: &GpuWorker, r1cs: &GpuR1cs) -> Result<(GpuParameters, GpuVerifyingKey), SynthesisError> {
+    generate_impl(worker, r1cs, ptr::null())
+}
