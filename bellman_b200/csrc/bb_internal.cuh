@@ -70,17 +70,12 @@ struct bb_ctx {
     long opt_msm_window_bits = 0;
     long opt_ntt_tile_log = 11;
     long opt_ntt_col_bits = 3;
-    long opt_ntt_radix8 = 0;          // 1 = register radix-8 windows (k_ntt_pass8) instead of the radix-2 sweeps in shared memory
     long opt_profile = 0;
-    long opt_msm_acc_variant = 0;     // accepted and ignored: the launch-bound / prefetch variants of round 1's accumulate kernel
-                                      // were removed
-    long opt_msm_reduce_2d = 1;      // bucket reduction through row / column sums (k_bucket_fold) for windows of >= 1024 buckets
     long opt_msm_reduce_k = 4;       // entries per thread and level of the bucket reduction: 4 halves the length of the
     long opt_msm_reduce_k1 = 4;      // dependent-addition chain of 16 (2K per level, log_K D levels) for 1.25x its additions
     long opt_msm_big_cap = 0;
     long opt_shard_windows = 4;      // multi-GPU: up to this many window shards per base range (1 = base ranges only)
     long opt_msm_affine_rounds = -1;  // batched-affine halving rounds per MSM: -1 = by size, 0 = none (XYZZ accumulation only)
-    long opt_msm_affine_tma = 0;      // dense halving rounds of G1 jobs: operands staged by cp.async.bulk + mbarrier (k_aff_phase3_tma)
     long opt_msm_affine_batch = 16;   // pairs per thread sharing one link of the inversion chain
     long opt_msm_precompute = 0;     // resident window multiples 2^(c w) P of every base vector (msm.cu: bases_build_table):
                                      // 1 = one bucket array per window slot, 2 = ONE bucket array for all windows

@@ -315,15 +315,21 @@ void bb_ctx_destroy(bb_ctx* ctx) {
     delete ctx;
 }
 
+// Options whose second implementation was measured slower than (or level with) the default path and then removed.
+// The keys stay accepted and have no effect, so that callers which still set them keep working.
+static bool retired_option(const std::string& k) {
+    for (const char* r : {"msm_acc_variant", "msm_affine_tma", "msm_reduce_2d", "ntt_radix8"})
+        if (k == r) return true;
+    return false;
+}
+
 int bb_ctx_set_option(bb_ctx* ctx, const char* key, long value) {
     if (!ctx || !key) { set_error("bb_ctx_set_option: null argument"); return BB_ERR_ARG; }
     std::string k(key);
     if (k == "msm_window_bits") ctx->opt_msm_window_bits = value;
     else if (k == "ntt_tile_log") ctx->opt_ntt_tile_log = value;
     else if (k == "ntt_col_bits") ctx->opt_ntt_col_bits = value;
-    else if (k == "ntt_radix8") ctx->opt_ntt_radix8 = value;
     else if (k == "profile") ctx->opt_profile = value;
-    else if (k == "msm_acc_variant") ctx->opt_msm_acc_variant = value;
     else if (k == "msm_big_cap") ctx->opt_msm_big_cap = value;
     else if (k == "msm_precompute") { if (value < 0 || value > 2) { set_error("msm_precompute is 0, 1 or 2"); return BB_ERR_ARG; } ctx->opt_msm_precompute = value; }
     else if (k == "msm_precompute_groups") { if (value < 0 || value > 3) { set_error("msm_precompute_groups is a mask of 1 (G1) and 2 (G2)"); return BB_ERR_ARG; } ctx->opt_msm_precompute_groups = value; }
@@ -332,11 +338,10 @@ int bb_ctx_set_option(bb_ctx* ctx, const char* key, long value) {
     else if (k == "params_read_chunk") { if (value < 1) { set_error("params_read_chunk >= 1"); return BB_ERR_ARG; } ctx->opt_params_read_chunk = value; }
     else if (k == "msm_affine_rounds") ctx->opt_msm_affine_rounds = value;
     else if (k == "msm_affine_batch") ctx->opt_msm_affine_batch = value;
-    else if (k == "msm_affine_tma") ctx->opt_msm_affine_tma = value;
-    else if (k == "msm_reduce_2d") ctx->opt_msm_reduce_2d = value;
     else if (k == "shard_windows") { if (value < 1) { set_error("shard_windows >= 1"); return BB_ERR_ARG; } ctx->opt_shard_windows = value; }
     else if (k == "msm_reduce_k1") { if (value < 2 || (value & (value - 1))) { set_error("msm_reduce_k1 must be a power of two >= 2"); return BB_ERR_ARG; } ctx->opt_msm_reduce_k1 = value; }
     else if (k == "msm_reduce_k") { if (value < 2 || (value & (value - 1))) { set_error("msm_reduce_k must be a power of two >= 2"); return BB_ERR_ARG; } ctx->opt_msm_reduce_k = value; }
+    else if (retired_option(k)) {}
     else { set_error("unknown option %s", key); return BB_ERR_ARG; }
     return BB_OK;
 }

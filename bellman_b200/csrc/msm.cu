@@ -30,7 +30,6 @@
 
 #include "bb_internal.cuh"
 #include "batch_affine.cuh"
-#include "tma.cuh"
 
 namespace bb {
 
@@ -679,7 +678,7 @@ int reduce_buckets_2d(bb_ctx* ctx, cudaStream_t st, XYZZ<F>* buckets, uint32_t W
                       DevBuf& d_fold, DevBuf& d_runs, DevBuf& d_partials, DevBuf& d_levels, XYZZ<F>* out) {
     uint32_t lg = 0;
     while ((1u << lg) < D) lg++;
-    if (!ctx->opt_msm_reduce_2d || D < 1024 || (1u << lg) != D) return reduce_buckets<F>(ctx, st, buckets, W, D, K0, K1, d_runs, d_partials, d_levels, out);
+    if (D < 1024 || (1u << lg) != D) return reduce_buckets<F>(ctx, st, buckets, W, D, K0, K1, d_runs, d_partials, d_levels, out);
     const uint32_t lo_bits = (lg + 1) / 2, Lo = 1u << lo_bits, H = D >> lo_bits;       // Lo >= H
     // small[0..W) = column sums (Lo each, weights lo + 1), small[W..2W) = row sums (H each, padded to Lo, weights hi)
     BB_TRY(d_fold.alloc(ctx, ((size_t)W * D / 2 + (size_t)W * D / 4 + (size_t)2 * W * Lo + 2 * (size_t)W) * sizeof(XYZZ<F>)));
@@ -737,81 +736,6 @@ static bool trace_on() { static int v = -1; if (v < 0) v = getenv("BB_TRACE") ? 
             fflush(stderr);                                                                       \
         }                                                                                         \
     } while (0)
-
-// ---- phase 3 of a DENSE halving round with the tiles staged by the copy engine ------------------------
-// In a dense round the CTA's pairs of iteration i are contiguous: rows 2 (i T + t0) ... of the previous
-// round's array (256 rows = 24 KB for G1) and prefixes i T + t0 ... (6 KB).  One elected thread asks the TMA
-// engine for both ranges (cp.async.bulk, completion on an mbarrier) one iteration ahead, into the other half
-// of a two-stage ring in shared memory; the warps only ever read operands from shared memory.  Same
-// arithmetic and the same results as k_aff_phase3<F, false>.
-template <class F>
-__global__ void __launch_bounds__(128) k_aff_phase3_tma(const Affine<F>* __restrict__ rows, const uint32_t* __restrict__ d_entries,
-                                                        uint32_t shift, size_t T, uint32_t L, const F* __restrict__ pre,
-                                                        const F* __restrict__ tp, Affine<F>* __restrict__ out) {
-    extern __shared__ uint4 shraw[];
-    __shared__ uint64_t bar[2];
-    constexpr uint32_t ROWS_BYTES = 256 * sizeof(Affine<F>), PRE_BYTES = 128 * sizeof(F), STAGE = ROWS_BYTES + PRE_BYTES;
-    char* smem = reinterpret_cast<char*>(shraw);
-    const size_t npairs = (size_t)(*d_entries) >> shift;
-    const size_t t0 = (size_t)blockIdx.x * 128, t = t0 + threadIdx.x;
-    if (t0 >= T || t0 >= npairs) return;                              // whole CTA without work (uniform)
-    const uint32_t nt = T - t0 < 128 ? (uint32_t)(T - t0) : 128u;
-    uint32_t cnt = (uint32_t)((npairs - t0 + T - 1) / T);             // iterations in which this CTA owns at least one pair
-    if (cnt > L) cnt = L;
-    if (threadIdx.x == 0) {
-        tma::mbar_init(&bar[0], 1);
-        tma::mbar_init(&bar[1], 1);
-        tma::mbar_fence_init();
-    }
-    __syncthreads();
-    auto issue = [&](uint32_t i, uint32_t s) {                        // thread 0 only
-        const size_t j0 = (size_t)i * T + t0;
-        const uint32_t valid = npairs - j0 < nt ? (uint32_t)(npairs - j0) : nt;
-        const uint32_t rb = valid * 2u * (uint32_t)sizeof(Affine<F>), pb = valid * (uint32_t)sizeof(F);
-        tma::mbar_arrive_expect_tx(&bar[s], rb + pb);
-        tma::bulk_g2s(smem + s * STAGE, rows + 2 * j0, rb, &bar[s]);
-        tma::bulk_g2s(smem + s * STAGE + ROWS_BYTES, pre + j0, pb, &bar[s]);
-    };
-    if (threadIdx.x == 0) issue(cnt - 1, 0);
-    const bool mine = t < T && t < npairs;
-    F run = mine ? ld_words(tp + t) : FieldOps<F>::one();
-    uint32_t parity[2] = {0, 0};
-    for (uint32_t k = 0; k < cnt; k++) {
-        const uint32_t i = cnt - 1 - k, s = k & 1u;
-        if (threadIdx.x == 0 && k + 1 < cnt) issue(i - 1, s ^ 1u);    // that half was released by the barrier below
-        tma::mbar_wait(&bar[s], parity[s]);
-        parity[s] ^= 1u;
-        const size_t j = (size_t)i * T + t;
-        if (mine && j < npairs) {
-            const Affine<F>* tile = reinterpret_cast<const Affine<F>*>(smem + s * STAGE);
-            Affine<F> P1 = ld_words(tile + 2 * threadIdx.x), P2 = ld_words(tile + 2 * threadIdx.x + 1);
-            const bool i1 = affine_is_identity(P1), i2 = affine_is_identity(P2);
-            if (i1 || i2) {
-                st_words(out + j, i1 ? P2 : P1);
-            } else {
-                F den = P2.x - P1.x, num;
-                bool skip = false;
-                if (den.is_zero()) {
-                    if (P1.y != P2.y || P1.y.is_zero()) { st_words(out + j, Affine<F>::identity()); skip = true; }
-                    else { den = P1.y.dbl(); F xx = P1.x.sqr(); num = xx.dbl() + xx; }
-                } else {
-                    num = P2.y - P1.y;
-                }
-                if (!skip) {
-                    const F* ptile = reinterpret_cast<const F*>(smem + s * STAGE + ROWS_BYTES);
-                    F inv = run * ld_words(ptile + threadIdx.x);
-                    run = run * den;
-                    F lam = num * inv;
-                    Affine<F> R;
-                    R.x = lam.sqr() - P1.x - P2.x;
-                    R.y = lam * (P1.x - R.x) - P1.y;
-                    st_words(out + j, R);
-                }
-            }
-        }
-        __syncthreads();                                              // everyone is done with stage s
-    }
-}
 
 // ---- upper levels of the batch inversion (batch_affine.cuh) ------------------------------------------
 template <class F>
@@ -1076,12 +1000,7 @@ int launch_msm(bb_msm_job* job) {
                 PairLoader<F, false> ld{bufs[(r - 1) & 1], nullptr};
                 k_aff_phase1<F, false><<<cdiv(T, 128), 128, 0, st>>>(ld, d_entries, r + 1, T, L, pre, tp);
                 BB_TRY(batch_invert_device<F>(ctx, st, tp, T, tp + T));
-                if (ctx->opt_msm_affine_tma && sizeof(F) == sizeof(Fp)) {        // G1: two 30 KB stages per CTA, three CTAs per SM
-                    const size_t sh_tma = 2 * (256 * sizeof(Affine<F>) + 128 * sizeof(F));
-                    BB_CUDA(cudaFuncSetAttribute(k_aff_phase3_tma<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh_tma));
-                    k_aff_phase3_tma<F><<<cdiv(T, 128), 128, sh_tma, st>>>(bufs[(r - 1) & 1], d_entries, r + 1, T, L, pre, tp, out);
-                } else
-                    k_aff_phase3<F, false><<<cdiv(T, 128), 128, 0, st>>>(ld, d_entries, r + 1, T, L, pre, tp, out, A.err);
+                k_aff_phase3<F, false><<<cdiv(T, 128), 128, 0, st>>>(ld, d_entries, r + 1, T, L, pre, tp, out, A.err);
             }
             ctx->count_launch(2);
             dense = out;
@@ -1538,7 +1457,7 @@ int bb_selftest_bucket_reduce(bb_ctx* ctx, const void* affine_pts, uint32_t D, u
     BB_TRY(d_b.alloc(ctx, D * sizeof(G1X))); BB_TRY(d_f.alloc(ctx, sizeof(G1X)));
     cudaStream_t st = ctx->main_stream;
     BB_CUDA(cudaMemcpyAsync(d_b.p, h.data(), D * sizeof(G1X), cudaMemcpyHostToDevice, st));
-    DevBuf d_fold;                                       // D >= 1024 takes the two-dimensional form unless msm_reduce_2d = 0
+    DevBuf d_fold;                                       // a power of two D >= 1024 takes the two-dimensional form
     BB_TRY(reduce_buckets_2d<Fp>(ctx, st, d_b.as<G1X>(), 1, D, K, K, d_fold, d_r, d_p, d_l, d_f.as<G1X>()));
     G1X r;
     BB_CUDA(cudaMemcpyAsync(&r, d_f.p, sizeof r, cudaMemcpyDeviceToHost, st));

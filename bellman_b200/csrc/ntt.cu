@@ -160,104 +160,6 @@ __global__ void __launch_bounds__(256) k_ntt_pass(PassArgs A) {
     }
 }
 
-// out-of-line Fr product for the fully unrolled radix-8 kernel: 12 inlined products per window made the kernel
-// ~15 K instructions and ncu showed it starved by instruction-cache misses (no_instruction 2.3 warps per issue)
-static __device__ __noinline__ Fr fr_mul_outlined(Fr a, Fr b) { return a * b; }
-
-// The same pass with radix-8 butterflies held in registers: a thread owns 8 elements that differ in three
-// consecutive row bits, runs those three stages on them without touching shared memory, and the tile is
-// exchanged through shared memory only between such windows (k = 8 stages: windows [0,3) [3,6) [5,8), the
-// last one running stages 6 and 7 only).  Two exchanges per pass instead of eight read-modify-write sweeps,
-// two barriers instead of nine; the first window reads global memory straight into registers and the last
-// one stores straight from them.  Twiddles: 7 per thread and window (1 + 2 + 4), read-only path.
-__global__ void __launch_bounds__(256) k_ntt_pass8(PassArgs A) {
-    extern __shared__ uint32_t sm[];
-    const size_t poff = (size_t)blockIdx.y * A.poly_stride;
-    const Fr* const src = A.src + poff;
-    Fr* const dst = A.dst + poff;
-    const Fr* const src_b = A.src_b ? A.src_b + poff : nullptr;
-    const Fr* const src_c = A.src_b ? A.src_c + poff : nullptr;
-    const uint32_t T = 1u << (A.k + A.cbits);
-    const uint32_t C = 1u << A.cbits;
-    const uint32_t hibits = A.cbits - A.lowbits;
-    const uint32_t blo_bits = A.s0 - A.lowbits;
-    const uint32_t B_lo = blockIdx.x & ((1u << blo_bits) - 1u);
-    const uint32_t B_hi = blockIdx.x >> blo_bits;
-    const uint32_t base_addr = (B_lo << A.lowbits) | (B_hi << (A.s0 + A.k + hibits));
-    const uint32_t lowmask = (1u << A.lowbits) - 1u;
-    auto addr = [&](uint32_t e) -> uint32_t {
-        uint32_t c = e & (C - 1u), r = e >> A.cbits;
-        return base_addr | (c & lowmask) | (r << A.s0) | ((c >> A.lowbits) << (A.s0 + A.k));
-    };
-    const uint32_t q = threadIdx.x;                      // T / 8 threads
-    const uint32_t nwin = (A.k + 2u) / 3u;
-    Fr x[8];
-    uint32_t done = 0;                                   // row bits whose stage has been run
-    for (uint32_t wi = 0; wi < nwin; wi++) {
-        uint32_t tw = 3u * wi;                           // window = row bits [tw, tw + 3)
-        if (tw + 3u > A.k) tw = A.k - 3u;
-        const uint32_t sh = A.cbits + tw;
-        const uint32_t e0 = ((q >> sh) << (sh + 3u)) | (q & ((1u << sh) - 1u));
-        if (wi == 0) {
-#pragma unroll
-            for (uint32_t u = 0; u < 8; u++) {
-                uint32_t p = addr(e0 | (u << sh));
-                uint32_t i = A.bitrev ? (__brev(p) >> (32u - A.log_n)) : p;
-                Fr v = ld_fr(src + i);
-                if (src_b) v = v * ld_fr(src_b + i) - ld_fr(src_c + i);
-                if (A.pre) v = v * ld_fr(A.pre + i);
-                x[u] = v;
-            }
-        } else {
-            __syncthreads();
-#pragma unroll
-            for (uint32_t u = 0; u < 8; u++) {
-                const uint32_t e = e0 | (u << sh);
-#pragma unroll
-                for (int w = 0; w < 8; w++) x[u].l[w] = sm[w * T + e];
-            }
-        }
-#pragma unroll
-        for (uint32_t lb = 0; lb < 3; lb++) {
-            const uint32_t t = tw + lb;
-            if (t < done) continue;                      // an overlapping window: this stage already ran
-            const uint32_t s = A.s0 + t;
-#pragma unroll
-            for (uint32_t u = 0; u < 8; u++) {
-                if (u & (1u << lb)) continue;
-                const uint32_t v = u | (1u << lb);
-                Fr y = x[v];
-                if (s != 0) {
-                    const uint32_t j = addr(e0 | (u << sh)) & ((1u << s) - 1u);
-                    y = fr_mul_outlined(y, ld_fr(A.tw + ((size_t)j << (A.log_n - s - 1u))));
-                }
-                Fr a = x[u];
-                x[u] = a + y;
-                x[v] = a - y;
-            }
-        }
-        done = tw + 3u;
-        if (wi + 1 < nwin) {
-            __syncthreads();                             // everyone has read the previous exchange
-#pragma unroll
-            for (uint32_t u = 0; u < 8; u++) {
-                const uint32_t e = e0 | (u << sh);
-#pragma unroll
-                for (int w = 0; w < 8; w++) sm[w * T + e] = x[u].l[w];
-            }
-        } else {
-#pragma unroll
-            for (uint32_t u = 0; u < 8; u++) {
-                const uint32_t p = addr(e0 | (u << sh));
-                Fr v = x[u];
-                if (A.post) v = v * ld_fr(A.post + p);
-                if (A.use_post_const) v = v * A.post_const;
-                st_fr(dst + p, v);
-            }
-        }
-    }
-}
-
 static Fr h_pow(const Fr& b, uint64_t e) { return b.pow_u64(e, fr_one()); }
 
 struct DomainConsts { Fr omega, omegainv, g, ginv, minv, zinv; };
@@ -375,12 +277,7 @@ static int run_passes(bb_ctx* ctx, cudaStream_t st, const Fr* src, Fr* data, Fr*
         if (smem > 48 * 1024) BB_CUDA(cudaFuncSetAttribute(k_ntt_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         const dim3 grid(1u << (log_n - k - cbits), polys);
         unsigned threads = (1u << (k + cbits)) / 2 < 256 ? ((1u << (k + cbits)) / 2 < 32 ? 32 : (1u << (k + cbits)) / 2) : 256;
-        // register radix-8 windows: 8 elements per thread, three row bits at a time (k >= 3), at least one warp per tile
-        const bool r8 = ctx->opt_ntt_radix8 && k >= 3 && (k + cbits) >= 8 && (k + cbits) <= 11;
-        if (r8) {
-            if (smem > 48 * 1024) BB_CUDA(cudaFuncSetAttribute(k_ntt_pass8, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            k_ntt_pass8<<<grid, (1u << (k + cbits)) / 8, smem, st>>>(A);
-        } else k_ntt_pass<<<grid, threads, smem, st>>>(A);
+        k_ntt_pass<<<grid, threads, smem, st>>>(A);
         ctx->count_launch();
         BB_CUDA(cudaGetLastError());
         s0 += k;

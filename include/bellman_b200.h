@@ -78,8 +78,6 @@ void bb_ctx_destroy(bb_ctx* ctx);
  *   msm_window_bits    window size c of the signed-digit Pippenger (0 = by size)
  *   msm_affine_rounds  batched-affine halving rounds before the XYZZ stage (-1 = by mean bucket fill, 0 = none)
  *   msm_affine_batch   pairs per thread in those rounds (default 16)
- *   msm_affine_tma     1 = dense rounds of G1 jobs staged by cp.async.bulk + mbarrier (default 0: measured neutral)
- *   msm_reduce_2d      0 = bucket reduction by the serial recursion over whole windows (default 1: row/column sums first)
  *   msm_reduce_k, msm_reduce_k1   entries per thread of the serial recursion (powers of two, default 4)
  *   msm_big_cap        bucket size above which a bucket is cut into tasks (0 = by mean fill)
  *   msm_precompute     keep window multiples of every base vector resident (see bb_bases_precompute): 1 = one bucket
@@ -90,9 +88,10 @@ void bb_ctx_destroy(bb_ctx* ctx);
  *   prove_batch_max    bb_groth16_prove_batch: at most this many proofs per sub-batch (0 = as many as memory allows)
  *   params_read_chunk  bb_params_read / bb_vk_read from host memory: staging bytes per chunk (default 64 MiB; rounded
  *                      down to whole points, at least one point)
- *   ntt_radix8         1 = register radix-8 NTT windows (default 0: measured slower), ntt_tile_log, ntt_col_bits
+ *   ntt_tile_log, ntt_col_bits   shape of the NTT tiles
  *   profile            1 = CUDA-event timing of the MSM stages, and of the verify.*, decode.*, r1cs.*, params.* and
- *                      generate.* stages (bb_profile_read) */
+ *                      generate.* stages (bb_profile_read)
+ *   msm_acc_variant, msm_affine_tma, msm_reduce_2d, ntt_radix8   retired: accepted for compatibility, no effect */
 int bb_ctx_set_option(bb_ctx* ctx, const char* key, long value);
 int bb_ctx_synchronize(bb_ctx* ctx);
 /* counters for the harness: number of kernels this context has launched */

@@ -255,17 +255,6 @@ void launch(bool cooperative, dim3 grid, dim3 block, size_t shmem, cudaStream_t,
 
 }  // namespace bb_emu
 
-// a fiber that polls something another fiber of the block will produce (mbarrier waits): back to the
-// scheduler, runnable again on its next sweep
-inline void bb_emu_yield() {
-    bb_emu::State& S = bb_emu::state();
-    if (!S.block || !S.cur) { std::fprintf(stderr, "cuda_emu: wait on a barrier in a kernel classified as barrier-free\n"); std::abort(); }
-    bb_emu::Fiber* f = S.cur;
-    f->wait_bar = nullptr;
-    swapcontext(&f->ctx, &S.sched);
-}
-#define BB_EMU_YIELD() bb_emu_yield()
-
 inline void bb_emu_need_block(const char* what) {
     if (!bb_emu::state().block) { std::fprintf(stderr, "cuda_emu: %s in a kernel build_emu.py classified as barrier-free\n", what); std::abort(); }
 }

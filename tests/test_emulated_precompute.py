@@ -71,18 +71,22 @@ def test_emulated_precompute_prove_and_shards(precompute):
 
 @pytest.mark.parametrize("variant", [33])
 def test_emulated_accumulate_variants(worker, variant):
-    """msm_acc_variant: round 1's launch-bound / prefetch variants of the accumulate kernel were measured (no gain) and removed;
-    the key is still accepted and changes nothing"""
-    worker.set_option("msm_acc_variant", variant)
-    try:
-        for pre in (0, 1):
-            worker.set_option("msm_precompute", pre)
-            G.test_multiexp_g1_matches_oracle(worker, 1000)
-            G.test_multiexp_g2_matches_oracle(worker, 40)
-            G.test_multiexp_error_semantics(worker)
-    finally:
-        worker.set_option("msm_acc_variant", 0)
-        worker.set_option("msm_precompute", 0)
+    """The retired options -- msm_acc_variant (round 1's launch-bound / prefetch variants of the accumulate kernel),
+    msm_affine_tma (bulk-copy staged halving rounds), msm_reduce_2d (bucket reduction without row / column sums) and
+    ntt_radix8 (register radix-8 NTT passes) -- selected second implementations that were measured (no gain) and removed;
+    each key, set away from its old default, is still accepted and changes nothing"""
+    retired = {"msm_acc_variant": (variant, 0), "msm_affine_tma": (1, 0), "msm_reduce_2d": (0, 1), "ntt_radix8": (1, 0)}
+    for key, (value, default) in retired.items():
+        worker.set_option(key, value)
+        try:
+            for pre in (0, 1):
+                worker.set_option("msm_precompute", pre)
+                G.test_multiexp_g1_matches_oracle(worker, 1000)
+                G.test_multiexp_g2_matches_oracle(worker, 40)
+                G.test_multiexp_error_semantics(worker)
+        finally:
+            worker.set_option(key, default)
+            worker.set_option("msm_precompute", 0)
 
 
 # ---- msm_precompute = 2: one bucket set for all windows ------------------------------------------------

@@ -106,9 +106,9 @@ def test_bucket_reduction_kernels(worker):
     """sum_d d * B_d (multiexp.rs:271-275) through the multi-level reduction, every level shape."""
     lib = bb.load_library()
     rng = random.Random(33)
-    for D, K, two_d in ((1, 8, 1), (2, 8, 1), (8, 8, 1), (64, 2, 1), (64, 8, 1), (512, 16, 1), (1024, 4, 1), (2048, 16, 1), (4096, 8, 1),
-                        (4096, 4, 0), (8192, 4, 1), (32768, 8, 0), (32768, 16, 1)):
-        worker.set_option("msm_reduce_2d", two_d)        # 1: windows of >= 1024 buckets go through row / column sums
+    # windows of >= 1024 buckets go through row / column sums first
+    for D, K in ((1, 8), (2, 8), (8, 8), (64, 2), (64, 8), (512, 16), (1024, 4), (2048, 16), (4096, 8),
+                 (4096, 4), (8192, 4), (32768, 8), (32768, 16)):
         ks = [rng.randrange(R) for _ in range(D)]
         for i in range(0, D, 7):
             ks[i] = 0                                   # empty buckets
@@ -118,14 +118,13 @@ def test_bucket_reduction_kernels(worker):
                                            out.ctypes.data_as(C.c_void_p))
         assert rc == 0
         want = o1.g1_fixed_mul(o1.fr_from_ints([sum((i + 1) * k for i, k in enumerate(ks)) % R]))
-        assert np.array_equal(out, want), (D, K, two_d)
-    worker.set_option("msm_reduce_2d", 1)
+        assert np.array_equal(out, want), (D, K)
 
 
 # --------------------------------------------------------------------------------------------
 # NTT (src/domain.rs)
 # --------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("log_n", [0, 1, 2, 3, 5, 8, 9, 11, 12, 13, 16])
+@pytest.mark.parametrize("log_n", [0, 1, 2, 3, 5, 8, 9, 10, 11, 12, 13, 14, 16])
 def test_ntt_matches_oracle(worker, log_n):
     o1.set_threads(8)
     v = o1.fr_random(100 + log_n, 1 << log_n)
@@ -149,23 +148,6 @@ def test_ntt_tile_shapes_do_not_change_results(worker):
     finally:
         worker.set_option("ntt_tile_log", 11)
         worker.set_option("ntt_col_bits", 3)
-
-
-def test_ntt_register_radix8_equals_radix2_sweeps(worker):
-    """k_ntt_pass8 (three stages per thread in registers) against k_ntt_pass (one stage per sweep of shared
-    memory) and the oracle, all four transforms, sizes whose passes split into 3+3+2, 3+3+1, 3+3, 3+2, 3 stages."""
-    try:
-        for log_n in (3, 5, 8, 10, 11, 12, 14):
-            v = o1.fr_random(300 + log_n, 1 << log_n)
-            for mode, omode in ((bb.NTT_FFT, o1.FFT), (bb.NTT_IFFT, o1.IFFT), (bb.NTT_COSET_FFT, o1.COSET_FFT), (bb.NTT_ICOSET_FFT, o1.ICOSET_FFT)):
-                want = o1.fft(v, omode)
-                for r8 in (1, 0):
-                    worker.set_option("ntt_radix8", r8)
-                    dom = bb.EvaluationDomain.from_coeffs(worker, v)
-                    [dom.fft, dom.ifft, dom.coset_fft, dom.icoset_fft][mode]()
-                    assert np.array_equal(dom.into_coeffs(), want), (log_n, mode, r8)
-    finally:
-        worker.set_option("ntt_radix8", 0)
 
 
 def test_ntt_padding_and_degree_limit(worker):
@@ -473,7 +455,8 @@ def affine(worker):
     worker.set_option("msm_affine_batch", 16)
 
 
-@pytest.mark.parametrize("n,rounds,batch", [(1, 3, 16), (2, 1, 16), (33, 2, 4), (1000, 3, 16), (1000, 1, 1), (3000, 4, 7), (1 << 14, 3, 16)])
+@pytest.mark.parametrize("n,rounds,batch", [(1, 3, 16), (2, 1, 16), (33, 2, 4), (1000, 3, 16), (1000, 1, 1), (3000, 4, 7), (5000, 3, 1),
+                                            (1 << 14, 3, 16)])
 def test_affine_rounds_g1_match_oracle(worker, affine, n, rounds, batch):
     affine(rounds, batch)
     ks = o1.fr_random(1000 + n, n)
@@ -549,21 +532,6 @@ def test_affine_rounds_special_pairs(worker, affine):
     e[kind == 1] = o1.fr_from_ints([1])[0]
     rc, want = o1.multiexp(1, b2, 7, dens.astype(np.uint8), e)
     assert rc == 0 and np.array_equal(_gpu_multiexp(worker, bb.G1, b2, 7, dens, e), want)
-
-
-def test_affine_rounds_tma_staged_variant(worker, affine):
-    """k_aff_phase3_tma (dense rounds fed by cp.async.bulk + mbarrier) gives the same points as the plain loads."""
-    try:
-        worker.set_option("msm_affine_tma", 1)
-        for n, rounds, batch in ((33, 2, 4), (1000, 3, 16), (3000, 4, 7), (5000, 3, 1)):
-            affine(rounds, batch)
-            bases = o1.g1_fixed_mul(o1.fr_random(1000 + n, n))
-            ex = o1.fr_random(2000 + n, n)
-            rc, want = o1.multiexp(1, bases, 0, None, ex)
-            assert rc == 0 and np.array_equal(_gpu_multiexp(worker, bb.G1, bases, 0, None, ex), want), (n, rounds, batch)
-        test_affine_rounds_special_pairs(worker, affine)
-    finally:
-        worker.set_option("msm_affine_tma", 0)
 
 
 def test_affine_rounds_error_semantics(worker, affine):
