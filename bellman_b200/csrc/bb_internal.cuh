@@ -181,6 +181,8 @@ struct StageTimer {
 inline unsigned cdiv(size_t a, size_t b) { return (unsigned)((a + b - 1) / b); }
 
 // ---- ntt.cu ----
+// The evaluation domain of n coefficients: m = 2^log_m >= n, or PolynomialDegreeTooLarge
+int domain_size(size_t n, size_t* m, uint32_t* log_m);
 int ntt_run_device(bb_ctx* ctx, cudaStream_t st, Fr* d_data, Fr* d_tmp, uint32_t log_n, int mode);
 int h_poly_device(bb_ctx* ctx, cudaStream_t st, Fr* d_a, Fr* d_b, Fr* d_c, Fr* d_tmp, uint32_t log_m);
 int h_poly_batch_device(bb_ctx* ctx, cudaStream_t st, Fr* d_abc, Fr* d_tmp, uint32_t log_m, uint32_t B);
@@ -266,19 +268,15 @@ int fixed_table_build(int group, const void* gen_affine, void** d_table);
 void fixed_table_free(int group, void* d_table);
 
 // ---- msm.cu ----
-struct MsmResult {
-    int status = BB_OK;
-    bool g2 = false;
-    G1X g1;
-    G2X x2;
-};
+// batch != 0: one job over `batch` scalar vectors (device memory, vector p at scalars + p * scalar_stride) sharing the
+// bases, the offset and the density map
 int msm_start(bb_ctx* ctx, const bb_bases* bases, size_t base_offset, const uint64_t* density_bits, size_t density_len,
               const void* scalars, bool scalars_on_device, size_t n, int form, cudaEvent_t wait_for, bb_msm_job** out,
               const char* tag = nullptr, int critical = 0, uint32_t batch = 0, size_t scalar_stride = 0);
-int msm_wait_result(bb_msm_job* job, MsmResult* res);
-// batch != 0: one job over `batch` scalar vectors (device memory, vector p at scalars + p * scalar_stride) sharing the
-// bases, the offset and the density map; msm_wait_batch gives each vector's status and folded point
-int msm_wait_batch(bb_msm_job* job, int* status, void* points);
+// Waits for a job and frees it.  For each scalar vector p (one for an unbatched job), status[p] is what bb_msm_wait would
+// report for that vector alone, and points[p] (G1X or G2X) its sum where status[p] is BB_OK.  Returns the job-level status
+// (a failure before or during the launch, or of the stream), which then stands for every vector.
+int msm_wait(bb_msm_job* job, int* status, void* points);
 size_t msm_batch_bytes(bb_ctx* ctx, const bb_bases* bases, size_t n, size_t n_dense, uint32_t batch, uint64_t* slots);
 int bases_build_table(bb_ctx* ctx, bb_bases* bases);
 // vals[i] <- 1 / vals[i] for n NON-ZERO field elements in HBM (Montgomery's trick, fan-in 32, one Fermat inversion);

@@ -464,13 +464,9 @@ int bb_domain_pointwise(bb_ctx* ctx, int op, void* fr_a_inout, const void* fr_b,
 int bb_h_poly(bb_ctx* ctx, const void* a, const void* b, const void* c, size_t n, void* h_out, size_t* m_out) {
     if (!ctx || !h_out || (n && (!a || !b || !c))) { set_error("bb_h_poly: null argument"); return BB_ERR_ARG; }
     BB_CUDA(cudaSetDevice(ctx->device));
-    size_t m = 1;
-    uint32_t log_m = 0;
-    while (m < n) {
-        m *= 2;
-        log_m++;
-        if (log_m >= (uint32_t)bbc::FR_S) { set_error("PolynomialDegreeTooLarge"); return BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE; }
-    }
+    size_t m;
+    uint32_t log_m;
+    BB_TRY(domain_size(n, &m, &log_m));
     DevBuf d_a, d_b, d_c, d_t;
     BB_TRY(d_a.alloc(ctx, m * 32)); BB_TRY(d_b.alloc(ctx, m * 32)); BB_TRY(d_c.alloc(ctx, m * 32)); BB_TRY(d_t.alloc(ctx, m * 32));
     cudaStream_t st = ctx->main_stream;

@@ -1282,10 +1282,7 @@ int classify_both_errors(bb_msm_job* job, uint32_t eof_index, int* status) {
     return BB_OK;
 }
 
-}  // namespace
-
-namespace bb {
-// profile mode: the job's stage times (accumulation, whole job, prover timeline) from its events, then the events go;
+// profile mode: the job's stage times (accumulation, whole job, prover timeline) from its events;
 // `cnt` = the job's counter words as copied back (err[4] pairs, err[5] bucket entries)
 void record_profile(bb_msm_job* job, int status, const uint32_t* cnt) {
     if (job->ev[3]) {
@@ -1314,70 +1311,39 @@ void record_profile(bb_msm_job* job, int status, const uint32_t* cnt) {
                 }
             }
         }
-        for (auto& e : job->ev) if (e) { cudaEventDestroy(e); e = nullptr; }
-        cudaGetLastError();
     }
 }
 
-// used by prover.cu: wait and return the projective result
-int msm_wait_result(bb_msm_job* job, MsmResult* res) {
-    int status = job->status;
-    {   // also on a failed launch: kernels already queued may still use the job's buffers
-        if (job->ev_done) { cudaEventSynchronize(job->ev_done); cudaEventDestroy(job->ev_done); job->ev_done = nullptr; }   // sleeps
-        cudaError_t e = cudaStreamSynchronize(job->st);                                                                     // returns at once after that
-        if (e != cudaSuccess && status == BB_OK) { set_error("msm stream: %s", cudaGetErrorString(e)); status = BB_ERR_CUDA; }
-    }
-    if (status == BB_OK) {
-        bool g2 = job->group == BB_G2;
-        size_t pts = (size_t)(job->W_out + 1) * (g2 ? sizeof(G2X) : sizeof(G1X));
-        const uint32_t* err = (const uint32_t*)((char*)job->h_out + pts);
-        bool eof = err[0] != 0xffffffffu, ident = err[1] != 0;
-        if (eof && ident) {
-            int s = g2 ? classify_both_errors<Fp2>(job, err[0], &status) : classify_both_errors<Fp>(job, err[0], &status);
-            if (s != BB_OK) status = s;
-        } else if (eof) {
-            status = BB_ERR_IO_UNEXPECTED_EOF;
-        } else if (ident) {
-            status = BB_ERR_UNEXPECTED_IDENTITY;
-        }
-        if (status == BB_ERR_IO_UNEXPECTED_EOF) set_error("expected more bases from source");
-        if (status == BB_ERR_UNEXPECTED_IDENTITY) set_error("encountered an identity element in the CRS");
-        if (status == BB_OK) {
-            res->g2 = g2;
-            const uint32_t wi = job->dargs.win_index, wc = job->dargs.win_count;
-            if (job->precomp) {                       // one window sum (weights already in the table) + the ones sum
-                if (g2) { res->x2 = ((const G2X*)job->h_out)[0]; res->x2.add(((const G2X*)job->h_out)[1]); }
-                else { res->g1 = ((const G1X*)job->h_out)[0]; res->g1.add(((const G1X*)job->h_out)[1]); }
-            } else if (g2) res->x2 = fold_windows<Fp2>((const G2X*)job->h_out, job->W, job->W_local, job->c, wi, wc);
-            else res->g1 = fold_windows<Fp>((const G1X*)job->h_out, job->W, job->W_local, job->c, wi, wc);
-        }
-    }
-    res->status = status;
-    record_profile(job, status, (const uint32_t*)((const char*)job->h_out + (size_t)(job->W_out + 1) * (job->group == BB_G2 ? sizeof(G2X) : sizeof(G1X))));
-    if (job->h_out) job->ctx->pinned_release(job->h_out);
-    delete job;
-    return status;
+// The job's result in `out`: the B device-folded points of a batched job, else the host fold of its window sums
+template <class F>
+void job_points(const bb_msm_job* job, XYZZ<F>* out) {
+    const XYZZ<F>* win = (const XYZZ<F>*)job->h_out;
+    if (job->batched) std::memcpy(out, win, job->B * sizeof(XYZZ<F>));
+    else if (job->precomp) { *out = win[0]; out->add(win[1]); }    // one window sum (weights already in the table) + the ones sum
+    else *out = fold_windows<F>(win, job->W, job->W_local, job->c, job->dargs.win_index, job->dargs.win_count);
 }
 
-// A batched job (msm_start with batch = B): for each proof p, status[p] is what msm_wait_result would report for that
-// vector alone, and points[p] (G1X or G2X) its folded sum where status[p] is BB_OK.  Returns the job-level status (a
-// failure before or during the launch, or of the stream), which then stands for every proof.  Frees the job.
-int msm_wait_batch(bb_msm_job* job, int* status, void* points) {
+}  // namespace
+
+namespace bb {
+int msm_wait(bb_msm_job* job, int* status, void* points) {
     int st = job->status;
-    if (job->ev_done) { cudaEventSynchronize(job->ev_done); cudaEventDestroy(job->ev_done); job->ev_done = nullptr; }
-    cudaError_t e = cudaStreamSynchronize(job->st);
+    // also on a failed launch: kernels already queued may still use the job's buffers
+    if (job->ev_done) { cudaEventSynchronize(job->ev_done); cudaEventDestroy(job->ev_done); job->ev_done = nullptr; }   // sleeps
+    cudaError_t e = cudaStreamSynchronize(job->st);                                                                     // returns at once after that
     if (e != cudaSuccess && st == BB_OK) { set_error("msm stream: %s", cudaGetErrorString(e)); st = BB_ERR_CUDA; }
     const uint32_t B = job->B;
     const bool g2 = job->group == BB_G2;
     const size_t psz = g2 ? sizeof(G2X) : sizeof(G1X);
+    // h_out: [B folded points] or [W_out window sums][ones sum], then err[8], then (batched) one identity word per vector
+    const uint32_t* err = job->h_out ? (const uint32_t*)((const char*)job->h_out + (job->batched ? B : job->W_out + 1) * psz) : nullptr;
     for (uint32_t p = 0; p < B; p++) status[p] = st;
-    if (st == BB_OK && job->h_out) {
-        const uint32_t* err = (const uint32_t*)((const char*)job->h_out + B * psz);
-        const uint32_t* perr = err + 8;
-        const bool eof = err[0] != 0xffffffffu;           // the shape alone decides it: the same for every proof
+    if (st == BB_OK && err) {
+        const bool eof = err[0] != 0xffffffffu;           // the shape alone decides it: the same for every vector
         for (uint32_t p = 0; p < B && st == BB_OK; p++) {
+            const bool ident = job->batched ? err[8 + p] != 0 : err[1] != 0;
             int s = BB_OK;
-            if (eof && perr[p]) {
+            if (eof && ident) {
                 const DigitArgs saved = job->dargs;
                 job->dargs.scalars += (size_t)p * saved.scalar_stride;
                 int c = g2 ? classify_both_errors<Fp2>(job, err[0], &s) : classify_both_errors<Fp>(job, err[0], &s);
@@ -1385,16 +1351,21 @@ int msm_wait_batch(bb_msm_job* job, int* status, void* points) {
                 if (c != BB_OK) st = c;
             } else if (eof) {
                 s = BB_ERR_IO_UNEXPECTED_EOF;
-            } else if (perr[p]) {
+            } else if (ident) {
                 s = BB_ERR_UNEXPECTED_IDENTITY;
             }
             status[p] = s;
         }
         if (st != BB_OK) for (uint32_t p = 0; p < B; p++) status[p] = st;
-        else std::memcpy(points, job->h_out, B * psz);
+        else if (job->batched || status[0] == BB_OK) {
+            if (g2) job_points<Fp2>(job, (G2X*)points);
+            else job_points<Fp>(job, (G1X*)points);
+        }
+        if (!job->batched && status[0] == BB_ERR_IO_UNEXPECTED_EOF) set_error("expected more bases from source");
+        if (!job->batched && status[0] == BB_ERR_UNEXPECTED_IDENTITY) set_error("encountered an identity element in the CRS");
     }
-    record_profile(job, st, job->h_out ? (const uint32_t*)((const char*)job->h_out + B * psz) : nullptr);
-    for (auto& ev : job->ev) if (ev) cudaEventDestroy(ev);      // the events of a job that failed before its last record
+    record_profile(job, job->batched ? st : status[0], err);
+    for (auto& ev : job->ev) if (ev) cudaEventDestroy(ev);      // also the events of a job that failed before its last record
     cudaGetLastError();
     if (job->h_out) job->ctx->pinned_release(job->h_out);
     delete job;
@@ -1438,10 +1409,12 @@ int bb_bases_drop_table(bb_bases* bases) {
 }
 int bb_msm_wait(bb_msm_job* job, void* out_affine) {
     if (!job || !out_affine) { set_error("bb_msm_wait: null argument"); return BB_ERR_ARG; }
-    MsmResult r;
-    int s = msm_wait_result(job, &r);
+    const bool g2 = job->group == BB_G2;
+    union { G1X g1; G2X g2; } r;
+    int s;
+    msm_wait(job, &s, &r);
     if (s != BB_OK) return s;
-    if (r.g2) { G2Affine a = r.x2.to_affine(); std::memcpy(out_affine, &a, sizeof a); }
+    if (g2) { G2Affine a = r.g2.to_affine(); std::memcpy(out_affine, &a, sizeof a); }
     else { G1Affine a = r.g1.to_affine(); std::memcpy(out_affine, &a, sizeof a); }
     return BB_OK;
 }

@@ -178,6 +178,17 @@ static DomainConsts domain_consts(uint32_t log_n) {
     return d;
 }
 
+int domain_size(size_t n, size_t* m, uint32_t* log_m) {
+    *m = 1;
+    *log_m = 0;
+    while (*m < n) {                                // from_coeffs, domain.rs:49-60
+        *m *= 2;
+        *log_m += 1;
+        if (*log_m >= (uint32_t)bbc::FR_S) { set_error("PolynomialDegreeTooLarge"); return BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE; }
+    }
+    return BB_OK;
+}
+
 enum TableKind { T_TW_FWD, T_TW_INV, T_POW_G, T_POW_GINV_MINV, T_POW_G_MINV, T_POW_GINV_MINV_ZINV };
 
 static int get_table(bb_ctx* ctx, cudaStream_t st, uint32_t log_n, TableKind kind, NttTables** tabs, const Fr** out) {
@@ -320,24 +331,8 @@ int ntt_run_device(bb_ctx* ctx, cudaStream_t st, Fr* d_data, Fr* d_tmp, uint32_t
 // prover.rs:225-237 on device buffers of m = 2^log_m elements (already zero padded).
 // Result (m coefficients, Montgomery) is left in d_a; d_b, d_c are clobbered.
 int h_poly_device(bb_ctx* ctx, cudaStream_t st, Fr* d_a, Fr* d_b, Fr* d_c, Fr* d_tmp, uint32_t log_m) {
-    if (log_m >= (uint32_t)bbc::FR_S) { set_error("2^%u-point domain: PolynomialDegreeTooLarge", log_m); return BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE; }
-    NttTables* t = nullptr;
-    const Fr *tw_f = nullptr, *tw_i = nullptr, *gm = nullptr, *gz = nullptr;
-    BB_TRY(get_table(ctx, st, log_m, T_TW_FWD, &t, &tw_f));
-    BB_TRY(get_table(ctx, st, log_m, T_TW_INV, &t, &tw_i));
-    BB_TRY(get_table(ctx, st, log_m, T_POW_G_MINV, &t, &gm));
-    BB_TRY(get_table(ctx, st, log_m, T_POW_GINV_MINV_ZINV, &t, &gz));
-    Fr* polys[3] = {d_a, d_b, d_c};
-    for (Fr* p : polys) {
-        Fusion inv;                     // ifft (:225,227,229) with the coset shift of :226,228,230 fused in
-        inv.post = gm;
-        BB_TRY(run_passes(ctx, st, p, p, d_tmp, log_m, tw_i, inv));
-        Fusion fwd;                     // the fft half of coset_fft
-        BB_TRY(run_passes(ctx, st, p, p, d_tmp, log_m, tw_f, fwd));
-    }
-    Fusion fin;                         // mul_assign, sub_assign, divide_by_z_on_coset, icoset_fft (:232-237)
-    fin.src_b = d_b; fin.src_c = d_c; fin.post = gz;
-    return run_passes(ctx, st, d_a, d_a, d_tmp, log_m, tw_i, fin);
+    for (Fr* p : {d_a, d_b, d_c}) BB_TRY(h_poly_evals_device(ctx, st, p, d_tmp, log_m));     // :225-230
+    return h_poly_final_device(ctx, st, d_a, d_b, d_c, d_tmp, log_m);                       // :232-237
 }
 
 // h_poly_device for B proofs in the same launches: d_abc holds a_0 .. a_{B-1}, b_0 .. b_{B-1}, c_0 .. c_{B-1}, m = 2^log_m

@@ -252,44 +252,97 @@ void batch_to_affine(const XYZZ<F>* in, size_t n, Affine<F>* out) {
     }
 }
 
+bool delta_is_identity(const bb_crs* crs) { return crs->delta_g1.is_identity() || crs->delta_g2.is_identity(); }     // prover.rs:320-324
+
 // The message bb_groth16_prove reports with status s for this key (NULL for the back-end statuses, whose text varies)
 const char* prove_status_message(const bb_crs* crs, int s) {
     switch (s) {
         case BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE: return "PolynomialDegreeTooLarge";
         case BB_ERR_UNEXPECTED_IDENTITY:
-            return crs->delta_g1.is_identity() || crs->delta_g2.is_identity() ? "delta is the identity: subversion-CRS attack"
-                                                                              : "encountered an identity element in the CRS";
+            return delta_is_identity(crs) ? "delta is the identity: subversion-CRS attack" : "encountered an identity element in the CRS";
         case BB_ERR_IO_UNEXPECTED_EOF: return "expected more bases from source";
         case BB_ERR_DENSITY_MISMATCH: return "density map length differs from the number of exponents";
         default: return nullptr;
     }
 }
 
-bool delta_is_identity(const bb_crs* crs) {                                       // prover.rs:320-324
-    if (!crs->delta_g1.is_identity() && !crs->delta_g2.is_identity()) return false;
-    set_error("delta is the identity: subversion-CRS attack");
-    return true;
+int prove_error(const bb_crs* crs, int s) {
+    if (const char* msg = prove_status_message(crs, s)) set_error("%s", msg);
+    return s;
+}
+
+// The status of one proof from its eight jobs' statuses st[k * stride] when several errors apply: the density assert fires
+// inside the multiexp() call itself (multiexp.rs:324-329; calls are made in slot order), the delta check comes before the
+// first wait (prover.rs:320-324), and the waits run a_inputs, a_aux, b_g1_inputs, b_g1_aux, b_g2_inputs, b_g2_aux, h, l
+// (:339-354).
+int proof_status(const int* st, size_t stride, bool bad_delta) {
+    static const int ref_wait_order[8] = {2, 3, 4, 5, 6, 7, 0, 1};
+    for (int k = 0; k < 8; k++) if (st[k * stride] == BB_ERR_DENSITY_MISMATCH) return BB_ERR_DENSITY_MISMATCH;
+    if (bad_delta) return BB_ERR_UNEXPECTED_IDENTITY;
+    for (int k : ref_wait_order) if (st[k * stride] != BB_OK) return st[k * stride];
+    return BB_OK;
+}
+
+size_t density_count(const uint64_t* bits, size_t n) {        // get_total_density, prover.rs:288-291
+    if (!bits) return n;
+    size_t c = 0;
+    for (size_t j = 0; j < (n + 63) / 64; j++) {
+        uint64_t wv = bits[j];
+        if (j == (n + 63) / 64 - 1 && (n & 63)) wv &= (1ull << (n & 63)) - 1ull;
+        c += (size_t)__builtin_popcountll(wv);
+    }
+    return c;
+}
+
+// The eight jobs of a proof in slot order: bases, base offset, density map, scalars, scalars the density selects, and the
+// device scalars of item i at src + i * stride Fr.  Slot 0 (h) takes its scalars from the H pipeline.
+struct Slot { const bb_bases* bases; size_t off; const uint64_t* dens; size_t n, n_dense; const void* src; size_t stride; };
+static const char* const job_tag[8] = {"h", "l", "a_inputs", "a_aux", "b_g1_inputs", "b_g1_aux", "b_g2_inputs", "b_g2_aux"};
+// h and the G2 job have the longest dependency chains: each gets one of the high-priority streams
+static const int job_critical[8] = {1, 0, 0, 0, 0, 0, 0, 2};
+
+void slot_table(const bb_crs* crs, const bb_witness& w, size_t m, const void* in, const void* aux, Slot out[8]) {
+    const size_t ni = w.n_inputs, na = w.n_aux, b_in = density_count(w.b_input_density, ni), b_aux = density_count(w.b_aux_density, na);
+    out[0] = {crs->h, 0, nullptr, m - 1, m - 1, nullptr, m};                                      // prover.rs:238-244
+    out[1] = {crs->l, 0, nullptr, na, na, aux, na};                                               // :263-268
+    out[2] = {crs->a, 0, nullptr, ni, ni, in, ni};                                                // :275-280
+    out[3] = {crs->a, ni, w.a_aux_density, na, density_count(w.a_aux_density, na), aux, na};      // :281-286
+    out[4] = {crs->b_g1, 0, w.b_input_density, ni, b_in, in, ni};                                 // :296-301
+    out[5] = {crs->b_g1, b_in, w.b_aux_density, na, b_aux, aux, na};                              // :302-307
+    out[6] = {crs->b_g2, 0, w.b_input_density, ni, b_in, in, ni};                                 // :312-317
+    out[7] = {crs->b_g2, b_in, w.b_aux_density, na, b_aux, aux, na};                              // :318
 }
 
 }  // namespace
 
-// One proof in flight: what prove_begin queued and prove_end collects.
+// B proofs of one shape in flight: one proof between prove_begin and prove_end (B = 1, unbatched jobs with host folds), or
+// a sub-batch of bb_groth16_prove_batch (batched jobs, one H pipeline for all items).  Every exit -- error paths included --
+// first drains every started job and the two streams that touch the buffers below (the DevBufs go back to the cache when
+// this object dies), then destroys the events.
 struct bb_prove {
-    bb_ctx* ctx = nullptr;
-    const bb_crs* crs = nullptr;
-    bb_witness w{};
-    size_t m = 1, b_in_total = 0;
-    uint32_t log_m = 0;
-    DevBuf d_a, d_b, d_c, d_tmp, d_in, d_aux;
+    bb_ctx* ctx;
+    const bb_crs* crs;
+    std::vector<bb_witness> w;
+    uint32_t B;
+    bool batched;
+    size_t m;
+    uint32_t log_m;
+    DevBuf d_abc, d_tmp, d_in, d_aux;             // d_abc: rows a_0 .. a_{B-1}, b_0 .., c_0 .. of m Fr; item i's h ends in a_i
     cudaStream_t up = nullptr;
     cudaEvent_t ev_up = nullptr, ev_h = nullptr;
-    bb_msm_job* jobs[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    int s = BB_OK;
+    Slot slot[8];
+    bb_msm_job* jobs[8] = {};
+    int s = BB_OK;                                // a failure to queue, reported at the end
     bool h_queued = false;
+    std::vector<int> status;                      // after prove_wait: item i's status in job k at [k * B + i] ...
+    std::vector<G1X> sums1;                       // ... and its point at [k * B + i] (k < 6) or [(k - 6) * B + i]
+    std::vector<G2X> sums2;
+    bb_prove(bb_ctx* c, const bb_crs* k, const bb_witness* items, uint32_t b, bool bat, size_t m_, uint32_t lm)
+        : ctx(c), crs(k), w(items, items + b), B(b), batched(bat), m(m_), log_m(lm) {}
     ~bb_prove() {
-        // every exit -- error paths included -- first drains every job and the two streams that touch the buffers
-        // above (the DevBufs go back to the cache when this object dies), then destroys the events
-        for (auto& j : jobs) if (j) { MsmResult r; msm_wait_result(j, &r); j = nullptr; }
+        std::vector<int> st(B);
+        std::vector<G2X> pts(B);
+        for (auto& j : jobs) if (j) { msm_wait(j, st.data(), pts.data()); j = nullptr; }
         if (ctx) cudaStreamSynchronize(ctx->main_stream);
         if (up) cudaStreamSynchronize(up);
         if (ev_up) cudaEventDestroy(ev_up);
@@ -299,169 +352,168 @@ struct bb_prove {
 
 namespace {
 
-static const char* const job_tag[8] = {"h", "l", "a_inputs", "a_aux", "b_g1_inputs", "b_g1_aux", "b_g2_inputs", "b_g2_aux"};
-
-void prove_start_job(bb_prove* P, int slot, const bb_bases* bases, size_t off, const uint64_t* dens, size_t dens_len, const void* d_sc, size_t cnt, cudaEvent_t ev) {
-    if (P->s == BB_OK)
-        P->s = msm_start(P->ctx, bases, off, dens, dens_len, d_sc, true, cnt, BB_FORM_MONTGOMERY, ev, &P->jobs[slot], job_tag[slot], slot == 0 ? 1 : slot == 7 ? 2 : 0);
+// profile mode: the origin of the jobs' device timeline (bb_profile_read "tl.<job>.<mark>")
+int profile_epoch(bb_ctx* ctx) {
+    if (!ctx->opt_profile) return BB_OK;
+    if (!ctx->epoch_ev) BB_CUDA(cudaEventCreate(&ctx->epoch_ev));
+    BB_CUDA(cudaEventRecord(ctx->epoch_ev, ctx->main_stream));
+    return BB_OK;
 }
 
-// The H pipeline (prover.rs:221-240) on the high-priority main stream and the h MSM behind it.  With `evals`
-// (device buffers of m coset evaluations of a, b, c -- computed elsewhere, bb_h_coset_evals) only the last
-// transform remains: mul_assign, sub_assign, divide_by_z_on_coset, icoset_fft (:232-237).
-int prove_queue_h(bb_prove* P, const void* const* evals) {
-    NvtxRange range(evals ? "bb: H pipeline (last transform) + h MSM" : "bb: H pipeline + h MSM");
+void prove_start(bb_prove* P, int k) {
+    const Slot& j = P->slot[k];
+    if (P->s == BB_OK)
+        P->s = msm_start(P->ctx, j.bases, j.off, j.dens, j.n, j.src, true, j.n, BB_FORM_MONTGOMERY, k == 0 ? P->ev_h : P->ev_up, &P->jobs[k],
+                         job_tag[k], job_critical[k], P->batched ? P->B : 0, j.stride);
+}
+
+// The H pipeline (prover.rs:221-240) of the B items on the high-priority main stream: a, b, c from the witnesses or from
+// `fill`, zero padded to m.  With `evals` (device buffers of m coset evaluations of a, b, c of one proof -- computed
+// elsewhere, bb_h_coset_evals) only the last transform remains: mul_assign, sub_assign, divide_by_z_on_coset, icoset_fft
+// (:232-237).
+int h_pipeline(bb_prove* P, const void* const* evals, const BatchAbcFill* fill) {
     bb_ctx* ctx = P->ctx;
     cudaStream_t st = ctx->main_stream;
-    const bb_witness* w = &P->w;
-    const size_t n = w->n_constraints, m = P->m;
-    const cudaMemcpyKind kind = w->on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    int s = BB_OK;
-    if (evals) {
-        s = h_poly_final_device(ctx, st, (Fr*)evals[0], (const Fr*)evals[1], (const Fr*)evals[2], P->d_tmp.as<Fr>(), P->log_m);
+    const bb_witness& w0 = P->w[0];
+    const size_t n = w0.n_constraints, m = P->m, B = P->B;
+    BB_TRY(P->d_tmp.alloc(ctx, (P->batched ? 3 * B : 1) * m * 32));
+    if (evals) return h_poly_final_device(ctx, st, (Fr*)evals[0], (const Fr*)evals[1], (const Fr*)evals[2], P->d_tmp.as<Fr>(), P->log_m);
+    BB_TRY(P->d_abc.alloc(ctx, 3 * B * m * 32));
+    Fr* abc = P->d_abc.as<Fr>();
+    if (fill) {                                          // a, b, c evaluated on the device from the uploaded witnesses
+        BB_CUDA(cudaStreamWaitEvent(st, P->ev_up, 0));
+        BB_TRY((*fill)(st, (uint32_t)B, abc, m, P->d_in.as<Fr>(), P->d_aux.as<Fr>()));
     } else {
-        auto stage = [&](DevBuf& d, const void* src) -> int {
-            if (m > n) BB_CUDA(cudaMemsetAsync((char*)d.p + n * 32, 0, (m - n) * 32, st));   // coeffs.resize(m, zero), domain.rs:69
-            if (n) BB_CUDA(cudaMemcpyAsync(d.p, src, n * 32, kind, st));
-            return BB_OK;
-        };
-        if (!w->on_device) ctx->h2d_bytes += 3 * n * 32;
-        if ((s = stage(P->d_a, w->a)) == BB_OK && (s = stage(P->d_b, w->b)) == BB_OK && (s = stage(P->d_c, w->c)) == BB_OK)
-            s = h_poly_device(ctx, st, P->d_a.as<Fr>(), P->d_b.as<Fr>(), P->d_c.as<Fr>(), P->d_tmp.as<Fr>(), P->log_m);
+        for (size_t i = 0; i < B; i++) {
+            const void* srcs[3] = {P->w[i].a, P->w[i].b, P->w[i].c};
+            for (size_t k = 0; k < 3 && n; k++)
+                BB_CUDA(cudaMemcpyAsync(abc + (k * B + i) * m, srcs[k], n * 32, w0.on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+        }
+        if (!w0.on_device) ctx->h2d_bytes += B * 3 * n * 32;
     }
-    if (s == BB_OK && cudaEventRecord(P->ev_h, st) != cudaSuccess) { set_error("cudaEventRecord(H pipeline done) failed"); s = BB_ERR_CUDA; }
+    if (m > n) BB_CUDA(cudaMemset2DAsync(abc + n, m * 32, 0, (m - n) * 32, 3 * B, st));   // coeffs.resize(m, zero), domain.rs:69
+    if (P->batched) return h_poly_batch_device(ctx, st, abc, P->d_tmp.as<Fr>(), P->log_m, (uint32_t)B);
+    return h_poly_device(ctx, st, abc, abc + m, abc + 2 * m, P->d_tmp.as<Fr>(), P->log_m);
+}
+
+// The H pipeline and the h MSM behind it
+int prove_queue_h(bb_prove* P, const void* const* evals, const BatchAbcFill* fill) {
+    NvtxRange range(evals ? "bb: H pipeline (last transform) + h MSM" : "bb: H pipeline + h MSM");
+    int s = h_pipeline(P, evals, fill);
+    if (s == BB_OK && cudaEventRecord(P->ev_h, P->ctx->main_stream) != cudaSuccess) { set_error("cudaEventRecord(H pipeline done) failed"); s = BB_ERR_CUDA; }
     if (s != BB_OK) { P->s = s; return s; }
-    prove_start_job(P, 0, P->crs->h, 0, nullptr, 0, evals ? evals[0] : P->d_a.p, m - 1, P->ev_h);             // :238-244
+    P->slot[0].src = evals ? evals[0] : P->d_abc.p;
+    prove_start(P, 0);
     P->h_queued = true;
     return P->s;
 }
 
-// Queues the uploads and the MSMs of one proof (prover.rs:221-318).  h_inline: the H pipeline and the h MSM are
-// queued here, FIRST -- they are the longest dependency chain of the proof and run on high-priority streams, the
-// seven witness MSMs fill the machine around them.  Otherwise prove_end queues them (multi-GPU: the coset
-// evaluations arrive from other ranks while the witness MSMs already run).
+// Queues the uploads and the MSMs of the B proofs (prover.rs:221-318).  h_inline: the H pipeline and the h MSM are queued
+// here, FIRST -- they are the longest dependency chain of a proof and run on high-priority streams, the seven witness MSMs
+// fill the machine around them.  Otherwise prove_end queues them (multi-GPU: the coset evaluations arrive from other ranks
+// while the witness MSMs already run).  A failure to queue a job is kept in P->s.
+int prove_queue(bb_prove* P, bool h_inline, const BatchAbcFill* fill) {
+    bb_ctx* ctx = P->ctx;
+    const bb_witness& w0 = P->w[0];
+    const size_t ni = w0.n_inputs, na = w0.n_aux, B = P->B;
+    BB_TRY(P->d_in.alloc(ctx, B * ni * 32)); BB_TRY(P->d_aux.alloc(ctx, B * na * 32));
+    P->up = ctx->pick_stream();
+    BB_CUDA(cudaEventCreateWithFlags(&P->ev_up, cudaEventDisableTiming));
+    BB_CUDA(cudaEventCreateWithFlags(&P->ev_h, cudaEventDisableTiming));
+    const cudaMemcpyKind kind = w0.on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    for (size_t i = 0; i < B; i++) {
+        if (ni) BB_CUDA(cudaMemcpyAsync((char*)P->d_in.p + i * ni * 32, P->w[i].input_assignment, ni * 32, kind, P->up));
+        if (na) BB_CUDA(cudaMemcpyAsync((char*)P->d_aux.p + i * na * 32, P->w[i].aux_assignment, na * 32, kind, P->up));
+    }
+    if (!w0.on_device) ctx->h2d_bytes += B * (ni + na) * 32;
+    BB_CUDA(cudaEventRecord(P->ev_up, P->up));
+    slot_table(P->crs, w0, P->m, P->d_in.p, P->d_aux.p, P->slot);
+    if (h_inline) prove_queue_h(P, nullptr, fill);
+    // all eight MSMs are in flight before the first wait (prover.rs:244-318); the G2 MSM has the longest chain of the seven
+    // (Fp2 arithmetic): it goes first, on the other high-priority stream
+    for (int k : {7, 1, 2, 3, 4, 5, 6}) prove_start(P, k);
+    return BB_OK;
+}
+
+// wait() x8 (prover.rs:339-354); always drains every started job.  The eight waits run on eight short-lived host threads:
+// jobs tend to finish together, and an unbatched job's wait ends with a host-side Horner fold of its window sums (255
+// doublings: 0.2 ms for G1, 0.5 ms for G2 on one core), so the folds overlap.  job_status[k]: job k's own status.
+void prove_wait(bb_prove* P, int job_status[8]) {
+    const size_t B = P->B;
+    P->status.assign(8 * B, BB_OK);
+    P->sums1.assign(6 * B, G1X::identity());
+    P->sums2.assign(2 * B, G2X::identity());
+    std::thread waiters[8];
+    for (int k = 0; k < 8; k++) {
+        job_status[k] = BB_OK;
+        bb_msm_job* job = P->jobs[k];
+        P->jobs[k] = nullptr;
+        if (!job) continue;
+        void* pts = k < 6 ? (void*)&P->sums1[k * B] : (void*)&P->sums2[(k - 6) * B];
+        waiters[k] = std::thread([=] {
+            cudaSetDevice(P->ctx->device);
+            job_status[k] = msm_wait(job, &P->status[k * B], pts);
+        });
+    }
+    for (auto& t : waiters) if (t.joinable()) t.join();
+}
+
+// The 960-byte partial sums of the listed items, to affine with one inversion for all their G1 points and one for all
+// their G2 points
+void write_partials(const bb_prove* P, const std::vector<uint32_t>& items, uint8_t* out) {
+    const size_t nk = items.size(), B = P->B;
+    std::vector<G1X> p1(6 * nk);
+    std::vector<G2X> p2(2 * nk);
+    for (size_t q = 0; q < nk; q++) {
+        for (size_t k = 0; k < 6; k++) p1[6 * q + k] = P->sums1[k * B + items[q]];
+        for (size_t k = 0; k < 2; k++) p2[2 * q + k] = P->sums2[k * B + items[q]];
+    }
+    std::vector<G1Affine> a1(6 * nk);
+    std::vector<G2Affine> a2(2 * nk);
+    batch_to_affine<Fp>(p1.data(), p1.size(), a1.data());
+    batch_to_affine<Fp2>(p2.data(), p2.size(), a2.data());
+    for (size_t q = 0; q < nk; q++) {
+        std::memcpy(out + q * BB_PARTIALS_BYTES, &a1[6 * q], 6 * 96);
+        std::memcpy(out + q * BB_PARTIALS_BYTES + 576, &a2[2 * q], 2 * 192);
+    }
+}
+
 int prove_begin_impl(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, bool h_inline, bb_prove** out) {
     NvtxRange range("bb: prove_begin (uploads, queue MSMs)");
     if (!ctx || !crs || !w || !out) { set_error("bb_groth16_prove: null argument"); return BB_ERR_ARG; }
     BB_CUDA(cudaSetDevice(ctx->device));
-    const size_t n = w->n_constraints;
-    size_t m = 1;
-    uint32_t log_m = 0;
-    while (m < n) {                                   // from_coeffs, domain.rs:49-60
-        m *= 2;
-        log_m += 1;
-        if (log_m >= (uint32_t)bbc::FR_S) { set_error("PolynomialDegreeTooLarge"); return BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE; }
-    }
-    cudaStream_t st = ctx->main_stream;
-    if (ctx->opt_profile) {                           // origin of the per-job device timeline (bb_profile_read "tl.<job>.<mark>")
-        if (!ctx->epoch_ev) BB_CUDA(cudaEventCreate(&ctx->epoch_ev));
-        BB_CUDA(cudaEventRecord(ctx->epoch_ev, st));
-    }
-    std::unique_ptr<bb_prove> P(new bb_prove());
-    P->ctx = ctx; P->crs = crs; P->w = *w; P->m = m; P->log_m = log_m;
-    if (h_inline) { BB_TRY(P->d_a.alloc(ctx, m * 32)); BB_TRY(P->d_b.alloc(ctx, m * 32)); BB_TRY(P->d_c.alloc(ctx, m * 32)); }
-    BB_TRY(P->d_tmp.alloc(ctx, m * 32));
-    BB_TRY(P->d_in.alloc(ctx, w->n_inputs * 32)); BB_TRY(P->d_aux.alloc(ctx, w->n_aux * 32));
-    P->up = ctx->pick_stream();
-    const cudaMemcpyKind kind = w->on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    if (w->n_inputs) BB_CUDA(cudaMemcpyAsync(P->d_in.p, w->input_assignment, w->n_inputs * 32, kind, P->up));
-    if (w->n_aux) BB_CUDA(cudaMemcpyAsync(P->d_aux.p, w->aux_assignment, w->n_aux * 32, kind, P->up));
-    if (!w->on_device) ctx->h2d_bytes += (w->n_inputs + w->n_aux) * 32;
-    BB_CUDA(cudaEventCreateWithFlags(&P->ev_up, cudaEventDisableTiming));
-    BB_CUDA(cudaEventCreateWithFlags(&P->ev_h, cudaEventDisableTiming));
-    BB_CUDA(cudaEventRecord(P->ev_up, P->up));
-    for (size_t j = 0; j < (w->n_inputs + 63) / 64; j++) {       // get_total_density, prover.rs:288-291
-        uint64_t wv = w->b_input_density[j];
-        if (j == (w->n_inputs + 63) / 64 - 1 && (w->n_inputs & 63)) wv &= (1ull << (w->n_inputs & 63)) - 1ull;
-        P->b_in_total += (size_t)__builtin_popcountll(wv);
-    }
-    bb_prove* p = P.get();
-    if (h_inline) prove_queue_h(p, nullptr);
-    const cudaEvent_t ev_up = P->ev_up;
-    const size_t b_in_total = P->b_in_total;
-    // all eight MSMs are in flight before the first wait (prover.rs:244-318); the G2 MSM has the longest chain
-    // of the seven (Fp2 arithmetic): it goes first, on the other high-priority stream
-    prove_start_job(p, 7, crs->b_g2, b_in_total, w->b_aux_density, w->n_aux, P->d_aux.p, w->n_aux, ev_up);      // :318
-    prove_start_job(p, 1, crs->l, 0, nullptr, 0, P->d_aux.p, w->n_aux, ev_up);                                  // :263-268
-    prove_start_job(p, 2, crs->a, 0, nullptr, 0, P->d_in.p, w->n_inputs, ev_up);                                // :275-280
-    prove_start_job(p, 3, crs->a, w->n_inputs, w->a_aux_density, w->n_aux, P->d_aux.p, w->n_aux, ev_up);        // :281-286
-    prove_start_job(p, 4, crs->b_g1, 0, w->b_input_density, w->n_inputs, P->d_in.p, w->n_inputs, ev_up);        // :296-301
-    prove_start_job(p, 5, crs->b_g1, b_in_total, w->b_aux_density, w->n_aux, P->d_aux.p, w->n_aux, ev_up);      // :302-307
-    prove_start_job(p, 6, crs->b_g2, 0, w->b_input_density, w->n_inputs, P->d_in.p, w->n_inputs, ev_up);        // :312-317
+    size_t m;
+    uint32_t log_m;
+    BB_TRY(domain_size(w->n_constraints, &m, &log_m));
+    BB_TRY(profile_epoch(ctx));
+    std::unique_ptr<bb_prove> P(new bb_prove(ctx, crs, w, 1, false, m, log_m));
+    BB_TRY(prove_queue(P.get(), h_inline, nullptr));
     *out = P.release();
-    return BB_OK;                                      // a failure to queue is kept in the state and reported by prove_end
+    return BB_OK;
 }
 
-// Queues the H pipeline if prove_begin did not, waits for the eight MSMs and writes the 960-byte partial sums.
-// Frees the state.  `while_device_runs`, if given, is called once everything is queued and before the first
-// wait: host work that needs no MSM result goes there and overlaps the device.
-int prove_end_impl(bb_prove* Praw, const void* const* evals, uint8_t* partials, const std::function<void()>* while_device_runs) {
+// Queues the H pipeline if prove_begin did not, waits for the eight MSMs and writes the 960-byte partial sums.  Frees the
+// state.
+int prove_end_impl(bb_prove* Praw, const void* const* evals, uint8_t* partials) {
     NvtxRange range("bb: prove_end (waits, folds)");
     std::unique_ptr<bb_prove> P(Praw);
     if (!Praw || !partials) { set_error("bb_groth16_prove_end: null argument"); return BB_ERR_ARG; }
-    bb_ctx* ctx = P->ctx;
-    const bb_crs* crs = P->crs;
-    BB_CUDA(cudaSetDevice(ctx->device));
-    if (!P->h_queued && P->s == BB_OK) {
-        if (!evals) { BB_TRY(P->d_a.alloc(ctx, P->m * 32)); BB_TRY(P->d_b.alloc(ctx, P->m * 32)); BB_TRY(P->d_c.alloc(ctx, P->m * 32)); }
-        prove_queue_h(P.get(), evals);
-    }
-    int s = P->s;
-    if (while_device_runs && *while_device_runs) (*while_device_runs)();
-    // wait() x8 (prover.rs:339-354); always drain every started job.  Each wait ends with a host-side Horner
-    // fold of the job's window sums (255 doublings: 0.2 ms for G1, 0.5 ms for G2 on one core); jobs tend to
-    // finish together, so the eight waits run on eight short-lived host threads and the folds overlap.
-    G1X sums1[6];
-    G2X sums2[2];
-    for (auto& p1 : sums1) p1 = G1X::identity();
-    for (auto& p2 : sums2) p2 = G2X::identity();
-    int slot_status[8] = {BB_OK, BB_OK, BB_OK, BB_OK, BB_OK, BB_OK, BB_OK, BB_OK};
-    {
-        std::thread waiters[8];
-        for (int k = 0; k < 8; k++) {
-            if (!P->jobs[k]) continue;
-            bb_msm_job* job = P->jobs[k];
-            P->jobs[k] = nullptr;
-            waiters[k] = std::thread([&, k, job] {
-                cudaSetDevice(ctx->device);
-                MsmResult r;
-                slot_status[k] = msm_wait_result(job, &r);
-                if (slot_status[k] == BB_OK) {
-                    if (k >= 6) sums2[k - 6] = r.x2;
-                    else sums1[k] = r.g1;
-                }
-            });
-        }
-        for (auto& t : waiters) if (t.joinable()) t.join();
-    }
-    if (s == BB_OK) {
-        // Which error create_proof reports when several apply: the density assert fires inside the
-        // multiexp() call itself (multiexp.rs:324-329; calls are made in slot order), the delta
-        // check comes before the first wait (prover.rs:320-324), and the waits run a_inputs, a_aux,
-        // b_g1_inputs, b_g1_aux, b_g2_inputs, b_g2_aux, h, l (:339-354).
-        static const int ref_wait_order[8] = {2, 3, 4, 5, 6, 7, 0, 1};
-        for (int k = 0; k < 8 && s == BB_OK; k++) if (slot_status[k] == BB_ERR_DENSITY_MISMATCH) s = slot_status[k];
-        if (s == BB_OK && delta_is_identity(crs)) s = BB_ERR_UNEXPECTED_IDENTITY;
-        for (int idx = 0; idx < 8 && s == BB_OK; idx++) s = slot_status[ref_wait_order[idx]];
-        // the message of the error that is reported (another job may have failed later)
-        if (const char* msg = prove_status_message(crs, s)) set_error("%s", msg);
-    }
-    if (s == BB_OK) {
-        G1Affine a1[6];
-        G2Affine a2[2];
-        batch_to_affine<Fp>(sums1, 6, a1);
-        batch_to_affine<Fp2>(sums2, 2, a2);
-        std::memcpy(partials, a1, 6 * 96);
-        std::memcpy(partials + 576, a2, 2 * 192);
-    }
-    return s;
+    BB_CUDA(cudaSetDevice(P->ctx->device));
+    if (!P->h_queued && P->s == BB_OK) prove_queue_h(P.get(), evals, nullptr);
+    int job_status[8];
+    prove_wait(P.get(), job_status);
+    if (P->s != BB_OK) return P->s;
+    const int s = proof_status(P->status.data(), 1, delta_is_identity(P->crs));
+    if (s != BB_OK) return prove_error(P->crs, s);
+    write_partials(P.get(), {0}, partials);
+    return BB_OK;
 }
 
-int prove_partials_impl(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, uint8_t* partials, const std::function<void()>* while_device_runs) {
+int prove_partials_impl(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, uint8_t* partials) {
     if (!partials) { set_error("bb_groth16_prove_partials: null argument"); return BB_ERR_ARG; }
     bb_prove* P = nullptr;
     BB_TRY(prove_begin_impl(ctx, crs, w, true, &P));
-    return prove_end_impl(P, nullptr, partials, while_device_runs);
+    return prove_end_impl(P, nullptr, partials);
 }
 
 // The terms of A, B, C that depend only on the key and on (r, s) -- prover.rs:326-337:
@@ -520,10 +572,10 @@ int finalize_impl(const bb_crs* crs, const uint8_t* partials, size_t count, cons
 
 
 // ---- many witnesses of one circuit against one key (bb_groth16_prove_batch) --------------------------------------------
-// A sub-batch of B items is one H pipeline per item on the main stream and EIGHT MSM jobs, each over the B scalar vectors of
-// its slot (msm_start with batch = B): the launches per sub-batch are those of one proof plus B - 1 H pipelines, and the
-// window folds run on the device.  The host work -- the scalar multiplications by r, s, rs -- is the single-proof code,
-// run for the items side by side.
+// A sub-batch of B items is one H pipeline for all items on the main stream and EIGHT MSM jobs, each over the B scalar
+// vectors of its slot (msm_start with batch = B): the launches per sub-batch are those of one proof plus B - 1 H pipelines,
+// and the window folds run on the device.  The host work -- the scalar multiplications by r, s, rs -- is the single-proof
+// code, run for the items side by side.
 
 // fn(i) for i < n on a pool of host threads, one per CPU this process may run on
 void parallel_for(size_t n, const std::function<void(size_t)>& fn) {
@@ -540,69 +592,16 @@ void parallel_for(size_t n, const std::function<void(size_t)>& fn) {
     for (auto& th : pool) th.join();
 }
 
-size_t density_count(const uint64_t* bits, size_t n) {
-    if (!bits) return n;
-    size_t c = 0;
-    for (size_t j = 0; j < (n + 63) / 64; j++) {
-        uint64_t wv = bits[j];
-        if (j == (n + 63) / 64 - 1 && (n & 63)) wv &= (1ull << (n & 63)) - 1ull;
-        c += (size_t)__builtin_popcountll(wv);
-    }
-    return c;
-}
-
 bool same_density(const uint64_t* a, const uint64_t* b, size_t bits) {
     if (!a || !b) return a == b;
     return std::memcmp(a, b, (bits + 63) / 64 * 8) == 0;
 }
 
-size_t domain_size(size_t n, uint32_t* log_m) {
-    size_t m = 1;
-    *log_m = 0;
-    while (m < n && *log_m < 63) { m *= 2; *log_m += 1; }
-    return m;
-}
-
-// One sub-batch in flight: the buffers of its B items and its eight jobs.  Every exit drains the jobs and the streams.
-struct BatchRun {
-    bb_ctx* ctx = nullptr;
-    uint32_t B = 0;
-    DevBuf d_in, d_aux, d_abc, d_tmp;
-    cudaStream_t up = nullptr;
-    cudaEvent_t ev_up = nullptr, ev_h = nullptr;
-    bb_msm_job* jobs[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    ~BatchRun() {
-        std::vector<int> st(B ? B : 1);
-        std::vector<G2X> pts(B ? B : 1);
-        for (auto& j : jobs) if (j) { msm_wait_batch(j, st.data(), pts.data()); j = nullptr; }
-        if (ctx) cudaStreamSynchronize(ctx->main_stream);
-        if (up) cudaStreamSynchronize(up);
-        if (ev_up) cudaEventDestroy(ev_up);
-        if (ev_h) cudaEventDestroy(ev_h);
-    }
-};
-
-// The eight jobs of a proof (bases, base offset, density, scalars, scalars the density selects) in slot order
-struct SlotShape { const bb_bases* bases; size_t off; const uint64_t* dens; size_t n; size_t n_dense; };
-void slot_shapes(const bb_crs* crs, const bb_witness* w, size_t m, SlotShape out[8]) {
-    const size_t b_in_total = density_count(w->b_input_density, w->n_inputs);
-    out[0] = {crs->h, 0, nullptr, m - 1, m - 1};
-    out[1] = {crs->l, 0, nullptr, w->n_aux, w->n_aux};
-    out[2] = {crs->a, 0, nullptr, w->n_inputs, w->n_inputs};
-    out[3] = {crs->a, w->n_inputs, w->a_aux_density, w->n_aux, density_count(w->a_aux_density, w->n_aux)};
-    out[4] = {crs->b_g1, 0, w->b_input_density, w->n_inputs, b_in_total};
-    out[5] = {crs->b_g1, b_in_total, w->b_aux_density, w->n_aux, density_count(w->b_aux_density, w->n_aux)};
-    out[6] = {crs->b_g2, 0, w->b_input_density, w->n_inputs, b_in_total};
-    out[7] = {crs->b_g2, b_in_total, w->b_aux_density, w->n_aux, density_count(w->b_aux_density, w->n_aux)};
-}
-
 // Proofs per sub-batch: prove_batch_max if set, and at most what one job's 2^32 bucket entries, its result staging block
 // and the device memory (free plus the context's cached blocks, against an estimate per proof) hold
-size_t batch_limit(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t count) {
-    uint32_t log_m;
-    const size_t m = domain_size(w->n_constraints, &log_m);
-    SlotShape js[8];
-    slot_shapes(crs, w, m, js);
+size_t batch_limit(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t m, size_t count) {
+    Slot js[8];
+    slot_table(crs, *w, m, nullptr, nullptr, js);
     size_t k = count;
     if (ctx->opt_prove_batch_max > 0) k = std::min(k, (size_t)ctx->opt_prove_batch_max);
     k = std::min(k, (bb_ctx::PINNED_BLOCK - 32) / (sizeof(G2X) + 4));
@@ -633,117 +632,32 @@ size_t batch_limit(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t c
 
 // Items 0 .. B - 1 of w: queue, wait, finalise.  Returns a failure of the sub-batch as a whole (it then stands for every
 // item); otherwise status[] holds each item's bb_groth16_prove status.
-int prove_sub_batch(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, uint32_t B, const uint8_t* r_bytes, const uint8_t* s_bytes,
-                    uint8_t* proofs, int* status, double* host_tail_ms, const BatchAbcFill* fill) {
-    const bb_witness& w0 = w[0];
-    const size_t n = w0.n_constraints, ni = w0.n_inputs, na = w0.n_aux;
-    uint32_t log_m;
-    const size_t m = domain_size(n, &log_m);
-    const cudaMemcpyKind kind = w0.on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    cudaStream_t st = ctx->main_stream;
-    BatchRun run;
-    run.ctx = ctx; run.B = B;
-    BB_TRY(run.d_abc.alloc(ctx, (size_t)3 * B * m * 32)); BB_TRY(run.d_tmp.alloc(ctx, (size_t)3 * B * m * 32));
-    BB_TRY(run.d_in.alloc(ctx, (size_t)B * ni * 32)); BB_TRY(run.d_aux.alloc(ctx, (size_t)B * na * 32));
-    run.up = ctx->pick_stream();
-    BB_CUDA(cudaEventCreateWithFlags(&run.ev_up, cudaEventDisableTiming));
-    BB_CUDA(cudaEventCreateWithFlags(&run.ev_h, cudaEventDisableTiming));
-    for (uint32_t i = 0; i < B; i++) {
-        if (ni) BB_CUDA(cudaMemcpyAsync((char*)run.d_in.p + (size_t)i * ni * 32, w[i].input_assignment, ni * 32, kind, run.up));
-        if (na) BB_CUDA(cudaMemcpyAsync((char*)run.d_aux.p + (size_t)i * na * 32, w[i].aux_assignment, na * 32, kind, run.up));
-    }
-    if (!w0.on_device) ctx->h2d_bytes += (size_t)B * (ni + na) * 32;
-    BB_CUDA(cudaEventRecord(run.ev_up, run.up));
-    // the H pipeline (prover.rs:221-240) of the whole sub-batch on the main stream: rows a_0 .. a_{B-1}, b_0 .., c_0 .. of
-    // m Fr, zero padded; item i's h coefficients are left in a_i
-    {
-        NvtxRange range("bb: batch H pipeline");
-        Fr* abc = run.d_abc.as<Fr>();
-        if (fill) {                                      // a, b, c evaluated on the device from the uploaded witnesses
-            BB_CUDA(cudaStreamWaitEvent(st, run.ev_up, 0));
-            BB_TRY((*fill)(st, B, abc, m, run.d_in.as<Fr>(), run.d_aux.as<Fr>()));
-        } else {
-            for (uint32_t i = 0; i < B; i++) {
-                const void* srcs[3] = {w[i].a, w[i].b, w[i].c};
-                for (uint32_t k = 0; k < 3 && n; k++)
-                    BB_CUDA(cudaMemcpyAsync(abc + ((size_t)k * B + i) * m, srcs[k], n * 32, kind, st));
-            }
-            if (!w0.on_device) ctx->h2d_bytes += (size_t)B * 3 * n * 32;
-        }
-        if (m > n) BB_CUDA(cudaMemset2DAsync(abc + n, m * 32, 0, (m - n) * 32, (size_t)3 * B, st));   // coeffs.resize(m, zero), domain.rs:69
-        BB_TRY(h_poly_batch_device(ctx, st, abc, run.d_tmp.as<Fr>(), log_m, B));
-        BB_CUDA(cudaEventRecord(run.ev_h, st));
-    }
-    SlotShape js[8];
-    slot_shapes(crs, &w0, m, js);
-    const void* src[8] = {run.d_abc.p, run.d_aux.p, run.d_in.p, run.d_aux.p, run.d_in.p, run.d_aux.p, run.d_in.p, run.d_aux.p};
-    const size_t stride[8] = {m, na, ni, na, ni, na, ni, na};
-    int s = BB_OK;
-    for (int slot : {0, 7, 1, 2, 3, 4, 5, 6}) {           // prove_begin's order: h, the G2 job, then the rest
-        const SlotShape& j = js[slot];
-        if (s == BB_OK)
-            s = msm_start(ctx, j.bases, j.off, j.dens, j.dens ? j.n : 0, src[slot], true, j.n, BB_FORM_MONTGOMERY, slot == 0 ? run.ev_h : run.ev_up,
-                          &run.jobs[slot], job_tag[slot], slot == 0 ? 1 : slot == 7 ? 2 : 0, B, stride[slot]);
-    }
-    if (s != BB_OK) return s;
+int prove_sub_batch(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, uint32_t B, size_t m, uint32_t log_m, const uint8_t* r_bytes,
+                    const uint8_t* s_bytes, uint8_t* proofs, int* status, double* host_tail_ms, const BatchAbcFill* fill) {
+    bb_prove P(ctx, crs, w, B, true, m, log_m);
+    BB_TRY(prove_queue(&P, true, fill));
+    if (P.s != BB_OK) return P.s;
     // while the device works: the MSM-independent terms of every item
     std::vector<ProofStatic> stat(B);
     std::vector<Fr> rr(B), ss(B);
     for (uint32_t i = 0; i < B; i++) { std::memcpy(rr[i].l, r_bytes + 32 * i, 32); std::memcpy(ss[i].l, s_bytes + 32 * i, 32); }
-    const bool bad_delta = crs->delta_g1.is_identity() || crs->delta_g2.is_identity();
+    const bool bad_delta = delta_is_identity(crs);
     if (!bad_delta) parallel_for(B, [&](size_t i) { finalize_static(crs, rr[i], ss[i], &stat[i]); });
-    std::vector<int> slot_status[8];
-    std::vector<G1X> sums1[6];
-    std::vector<G2X> sums2[2];
-    int job_status[8] = {BB_OK, BB_OK, BB_OK, BB_OK, BB_OK, BB_OK, BB_OK, BB_OK};
-    {
-        std::thread waiters[8];
-        for (int k = 0; k < 8; k++) {
-            slot_status[k].assign(B, BB_OK);
-            if (k < 6) sums1[k].assign(B, G1X::identity()); else sums2[k - 6].assign(B, G2X::identity());
-            bb_msm_job* job = run.jobs[k];
-            run.jobs[k] = nullptr;
-            if (!job) continue;
-            waiters[k] = std::thread([&, k, job] {
-                cudaSetDevice(ctx->device);
-                void* pts = k < 6 ? (void*)sums1[k].data() : (void*)sums2[k - 6].data();
-                job_status[k] = msm_wait_batch(job, slot_status[k].data(), pts);
-            });
-        }
-        for (auto& th : waiters) if (th.joinable()) th.join();
-    }
+    int job_status[8];
+    prove_wait(&P, job_status);
     const auto t_waited = std::chrono::steady_clock::now();
     // the density assert is a per-item status; anything else a job failed with is the sub-batch's
     for (int k = 0; k < 8; k++) if (job_status[k] != BB_OK && job_status[k] != BB_ERR_DENSITY_MISMATCH) return job_status[k];
-    // each item's status as prove_end_impl decides it for a single proof
-    static const int ref_wait_order[8] = {2, 3, 4, 5, 6, 7, 0, 1};
     std::vector<uint32_t> ok;
     for (uint32_t i = 0; i < B; i++) {
-        int si = BB_OK;
-        for (int k = 0; k < 8 && si == BB_OK; k++) if (slot_status[k][i] == BB_ERR_DENSITY_MISMATCH) si = BB_ERR_DENSITY_MISMATCH;
-        if (si == BB_OK && bad_delta) si = BB_ERR_UNEXPECTED_IDENTITY;
-        for (int idx = 0; idx < 8 && si == BB_OK; idx++) si = slot_status[ref_wait_order[idx]][i];
-        status[i] = si;
-        if (si == BB_OK) ok.push_back(i);
+        status[i] = proof_status(&P.status[i], B, bad_delta);
+        if (status[i] == BB_OK) ok.push_back(i);
     }
-    // to affine: one inversion for all G1 points of the sub-batch and one for all G2 points
-    const size_t nk = ok.size();
-    std::vector<G1X> p1(6 * nk);
-    std::vector<G2X> p2(2 * nk);
-    for (size_t q = 0; q < nk; q++) {
-        for (int k = 0; k < 6; k++) p1[6 * q + k] = sums1[k][ok[q]];
-        for (int k = 0; k < 2; k++) p2[2 * q + k] = sums2[k][ok[q]];
-    }
-    std::vector<G1Affine> a1(6 * nk);
-    std::vector<G2Affine> a2(2 * nk);
-    batch_to_affine<Fp>(p1.data(), p1.size(), a1.data());
-    batch_to_affine<Fp2>(p2.data(), p2.size(), a2.data());
-    parallel_for(nk, [&](size_t q) {
+    std::vector<uint8_t> partials(ok.size() * BB_PARTIALS_BYTES);
+    write_partials(&P, ok, partials.data());
+    parallel_for(ok.size(), [&](size_t q) {
         const uint32_t i = ok[q];
-        uint8_t partials[BB_PARTIALS_BYTES];
-        std::memcpy(partials, &a1[6 * q], 6 * 96);
-        std::memcpy(partials + 576, &a2[2 * q], 2 * 192);
-        finalize_impl(crs, partials, 1, rr[i], ss[i], stat[i], proofs + (size_t)i * BB_PROOF_BYTES);
+        finalize_impl(crs, &partials[q * BB_PARTIALS_BYTES], 1, rr[i], ss[i], stat[i], proofs + (size_t)i * BB_PROOF_BYTES);
     });
     *host_tail_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_waited).count();
     return BB_OK;
@@ -782,25 +696,21 @@ int prove_batch_impl(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t
         }
     }
     std::memset(proofs, 0, count * BB_PROOF_BYTES);
+    size_t m;
     uint32_t log_m;
-    domain_size(w0.n_constraints, &log_m);
-    if (log_m >= (uint32_t)bbc::FR_S) {                   // from_coeffs, domain.rs:49-60: every item alike
-        set_error("%s", prove_status_message(crs, BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE));
+    if (domain_size(w0.n_constraints, &m, &log_m) != BB_OK) {     // every item alike
         for (size_t i = 0; i < count; i++) status[i] = BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE;
         return BB_OK;
     }
     BB_CUDA(cudaSetDevice(ctx->device));
     NvtxRange range("bb: prove_batch");
-    if (ctx->opt_profile) {                           // origin of the jobs' device timeline (bb_profile_read "tl.<job>.<mark>")
-        if (!ctx->epoch_ev) BB_CUDA(cudaEventCreate(&ctx->epoch_ev));
-        BB_CUDA(cudaEventRecord(ctx->epoch_ev, ctx->main_stream));
-    }
-    const size_t k = batch_limit(ctx, crs, &w0, count);
+    BB_TRY(profile_epoch(ctx));
+    const size_t k = batch_limit(ctx, crs, &w0, m, count);
     double tail = 0;
     size_t subs = 0;
     for (size_t lo = 0; lo < count; lo += k, subs++) {
         const uint32_t B = (uint32_t)std::min(k, count - lo);
-        const int rc = prove_sub_batch(ctx, crs, w + lo, B, r + 32 * lo, s + 32 * lo, proofs + lo * BB_PROOF_BYTES, status + lo, &tail, fill);
+        const int rc = prove_sub_batch(ctx, crs, w + lo, B, m, log_m, r + 32 * lo, s + 32 * lo, proofs + lo * BB_PROOF_BYTES, status + lo, &tail, fill);
         for (uint32_t i = 0; i < B; i++) {
             if (rc != BB_OK) status[lo + i] = rc;          // a failure of the sub-batch as a whole: none of its items has a proof
             if (status[lo + i] != BB_OK) std::memset(proofs + (lo + i) * BB_PROOF_BYTES, 0, BB_PROOF_BYTES);
@@ -817,7 +727,7 @@ int prove_batch_impl(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t
 extern "C" {
 
 int bb_groth16_prove_partials(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, uint8_t* partials) {
-    return prove_partials_impl(ctx, crs, w, partials, nullptr);
+    return prove_partials_impl(ctx, crs, w, partials);
 }
 
 int bb_groth16_prove_begin(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, bb_prove** out) {
@@ -828,7 +738,7 @@ int bb_groth16_prove_end(bb_prove* state, const void* d_evals_a, const void* d_e
     const bool any = d_evals_a || d_evals_b || d_evals_c;
     if (any && !(d_evals_a && d_evals_b && d_evals_c)) { delete state; set_error("bb_groth16_prove_end: all three evaluation vectors or none"); return BB_ERR_ARG; }
     const void* ev[3] = {d_evals_a, d_evals_b, d_evals_c};
-    return prove_end_impl(state, any ? ev : nullptr, partials, nullptr);
+    return prove_end_impl(state, any ? ev : nullptr, partials);
 }
 
 // from_coeffs (zero padding to m), ifft and coset_fft of ONE of the polynomials a, b, c (prover.rs:225-230) into a
@@ -837,13 +747,9 @@ int bb_groth16_prove_end(bb_prove* state, const void* d_evals_a, const void* d_e
 int bb_h_coset_evals_async(bb_ctx* ctx, const void* poly, size_t n_constraints, int on_device, void* d_out) {
     if (!ctx || !d_out || (n_constraints && !poly)) { set_error("bb_h_coset_evals: null argument"); return BB_ERR_ARG; }
     BB_CUDA(cudaSetDevice(ctx->device));
-    size_t m = 1;
-    uint32_t log_m = 0;
-    while (m < n_constraints) {
-        m *= 2;
-        log_m += 1;
-        if (log_m >= (uint32_t)bbc::FR_S) { set_error("PolynomialDegreeTooLarge"); return BB_ERR_POLYNOMIAL_DEGREE_TOO_LARGE; }
-    }
+    size_t m;
+    uint32_t log_m;
+    BB_TRY(domain_size(n_constraints, &m, &log_m));
     cudaStream_t st = ctx->main_stream;
     void* d_tmp = nullptr;
     BB_TRY(ctx->alloc(m * 32, &d_tmp));
@@ -880,7 +786,7 @@ int bb_h_coset_evals(bb_ctx* ctx, const void* poly, size_t n_constraints, int on
 int bb_groth16_finalize(const bb_crs* crs, const uint8_t* partials, size_t count, const uint8_t* r_bytes, const uint8_t* s_bytes,
                         uint8_t* proof) {
     if (!crs || !partials || !count || !r_bytes || !s_bytes || !proof) { set_error("bb_groth16_finalize: null argument"); return BB_ERR_ARG; }
-    if (delta_is_identity(crs)) return BB_ERR_UNEXPECTED_IDENTITY;
+    if (delta_is_identity(crs)) return prove_error(crs, BB_ERR_UNEXPECTED_IDENTITY);
     Fr r, s;
     std::memcpy(r.l, r_bytes, 32);
     std::memcpy(s.l, s_bytes, 32);
@@ -905,7 +811,7 @@ int bb_groth16_finalize_static(const bb_crs* crs, const uint8_t* r_bytes, const 
 int bb_groth16_finalize_with(const bb_crs* crs, const uint8_t* partials, size_t count, const uint8_t* r_bytes, const uint8_t* s_bytes,
                              const uint8_t* static_in, uint8_t* proof) {
     if (!crs || !partials || !count || !r_bytes || !s_bytes || !static_in || !proof) { set_error("bb_groth16_finalize_with: null argument"); return BB_ERR_ARG; }
-    if (delta_is_identity(crs)) return BB_ERR_UNEXPECTED_IDENTITY;
+    if (delta_is_identity(crs)) return prove_error(crs, BB_ERR_UNEXPECTED_IDENTITY);
     Fr r, s;
     std::memcpy(r.l, r_bytes, 32);
     std::memcpy(s.l, s_bytes, 32);
@@ -991,7 +897,7 @@ int bb_groth16_autotune(bb_ctx* ctx, bb_crs* crs, const bb_witness* w, int reps,
         int s = bb_crs_apply_tuning(ctx, crs, i);
         if (s != BB_OK) { if (i == 0) return s; continue; }
         std::memset(got, 0, sizeof got);
-        s = prove_partials_impl(ctx, crs, w, got, nullptr);             // first proof of this form: builds caches, checked
+        s = prove_partials_impl(ctx, crs, w, got);             // first proof of this form: builds caches, checked
         if (s != BB_OK) {
             if (i == 0) return s;                       // the witness / key itself fails: nothing to tune
             ms[i] = -2.0;                               // -2: this form failed where the default did not
@@ -1002,7 +908,7 @@ int bb_groth16_autotune(bb_ctx* ctx, bb_crs* crs, const bb_witness* w, int reps,
         double fastest = 1e300;
         for (int k = 0; k < reps && s == BB_OK; k++) {
             const auto t0 = std::chrono::steady_clock::now();
-            s = prove_partials_impl(ctx, crs, w, got, nullptr);
+            s = prove_partials_impl(ctx, crs, w, got);
             const double dt = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
             if (dt < fastest) fastest = dt;
         }
@@ -1023,19 +929,17 @@ int bb_groth16_prove(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, const 
     Fr r, s;
     std::memcpy(r.l, r_bytes, 32);
     std::memcpy(s.l, s_bytes, 32);
-    // the five scalar multiplications that need no MSM result run on the host while the device works
-    ProofStatic stat;
-    const bool bad_delta = crs->delta_g1.is_identity() || crs->delta_g2.is_identity();
     // profile mode: host-side milestones of one prove, ms since entry (bb_profile_read "host.<mark>")
     const auto t_entry = std::chrono::steady_clock::now();
     auto since = [&] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_entry).count(); };
-    double t_queued = 0, t_static = 0;
-    std::function<void()> overlap = [&] {
-        t_queued = since();
-        if (!bad_delta) finalize_static(crs, r, s, &stat);
-        t_static = since();
-    };
-    BB_TRY(prove_partials_impl(ctx, crs, w, partials, &overlap));     // reports delta = identity as well (prover.rs:320-324)
+    bb_prove* P = nullptr;
+    BB_TRY(prove_begin_impl(ctx, crs, w, true, &P));
+    const double t_queued = since();
+    // the five scalar multiplications that need no MSM result run on the host while the device works
+    ProofStatic stat;
+    if (!delta_is_identity(crs)) finalize_static(crs, r, s, &stat);
+    const double t_static = since();
+    BB_TRY(prove_end_impl(P, nullptr, partials));     // reports delta = identity as well (prover.rs:320-324)
     const double t_waited = since();
     int rc = finalize_impl(crs, partials, 1, r, s, stat, proof);
     if (ctx && ctx->opt_profile) {

@@ -282,7 +282,7 @@ int verify_batch(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* b, const vo
     c_bases.ctx = ctx; c_bases.group = BB_G1; c_bases.d_points = (void*)d_c; c_bases.n = n; c_bases.global_offset = 0; c_bases.global_len = n;
     bb_msm_job* jobs[2] = {nullptr, nullptr};
     auto drain = [&]() {                                         // every exit waits for the jobs that use this call's buffers
-        for (auto& j : jobs) if (j) { MsmResult r; msm_wait_result(j, &r); j = nullptr; }
+        for (auto& j : jobs) if (j) { int sj; G1X pj; msm_wait(j, &sj, &pj); j = nullptr; }
         if (c_bases.d_table) { ctx->release(c_bases.d_table); c_bases.d_table = nullptr; }
         if (ev_scalars) { cudaEventDestroy(ev_scalars); ev_scalars = nullptr; }
     };
@@ -302,17 +302,18 @@ int verify_batch(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* b, const vo
     ctx->count_launch();
     tm.mark("verify.miller");
 
-    MsmResult res[2];
+    G1X res[2];
     int status = BB_OK;
     for (int k = 0; k < 2; k++) {
-        int sk = msm_wait_result(jobs[k], &res[k]);
+        int sk;
+        msm_wait(jobs[k], &sk, &res[k]);
         jobs[k] = nullptr;
         if (status == BB_OK) status = sk;
     }
     drain();
     if (status != BB_OK) { cudaStreamSynchronize(st); return status; }
     tm.mark("verify.msm_wait");
-    G1Eval h_pe[2] = {g1_eval_from_xyzz(res[0].g1), g1_eval_from_xyzz(res[1].g1)};      // (acc_Delta, delta), (Psi, gamma)
+    G1Eval h_pe[2] = {g1_eval_from_xyzz(res[0]), g1_eval_from_xyzz(res[1])};      // (acc_Delta, delta), (Psi, gamma)
     BB_CUDA(cudaMemcpyAsync(d_pev + n, h_pe, sizeof h_pe, cudaMemcpyHostToDevice, st));
     k_miller<<<1, 3, 0, st>>>(d_pev + n, d_qv + n, 3, d_f.as<Fp12>() + n);
     ctx->count_launch();
