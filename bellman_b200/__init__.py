@@ -740,7 +740,7 @@ from .verifier import (BatchVerifier, InvalidProof, InvalidVerifyingKey, Prepare
 # Proof::read / Proof::write over a batch (groth16/src/lib.rs:39-99)
 from .verifier import InvalidProofEncoding, read_proof, read_proofs, write_proofs  # noqa: E402
 # the constraint system on the device: prove from the witness alone (groth16/src/prover.rs:19-55,105-145)
-from .r1cs import (R1CS, create_proof_r1cs, create_proof_r1cs_batch, create_random_proof_r1cs,  # noqa: E402
+from .r1cs import (R1CS, check_r1cs_batch, create_proof_r1cs, create_proof_r1cs_batch, create_random_proof_r1cs,  # noqa: E402
                    create_random_proof_r1cs_batch)
 # Parameters::read / VerifyingKey::read on the device (groth16/src/lib.rs:158-218, 289-398)
 from .params_io import InvalidData, read_parameters_device, read_verifying_key_device  # noqa: E402

@@ -81,6 +81,19 @@ __global__ void __launch_bounds__(GROUP_THREADS) k_r1cs_rows_group(EvalArgs A, c
     if (lane == 0 && slot < count) r1cs_put(A, g, sh[threadIdx.x]);
 }
 
+// which_is_unsatisfied over evaluated rows: row k fails when a[k] b[k] != c[k] (Montgomery product, limb equality; every
+// value is below r).  A failing row lowers *first, counts itself in *count and, with bits, sets bit k of the LSB-first
+// words (the uint64 density words' bytes).  A satisfied witness issues no atomics.
+__global__ void __launch_bounds__(256) k_r1cs_check(const Fr* __restrict__ a, const Fr* __restrict__ b, const Fr* __restrict__ c,
+                                                    uint32_t n, uint32_t* __restrict__ first, uint32_t* __restrict__ count,
+                                                    uint32_t* __restrict__ bits) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n || a[k] * b[k] == c[k]) return;
+    atomicMin(first, k);
+    atomicAdd(count, 1u);
+    if (bits) atomicOr(bits + k / 32, 1u << (k % 32));
+}
+
 bool fr_geq_modulus(const uint32_t* v) {
     for (int i = 7; i >= 0; i--) {
         if (v[i] > bbc::FR_MOD[i]) return true;
@@ -136,6 +149,64 @@ int r1cs_eval_queue(bb_ctx* ctx, cudaStream_t st, const bb_r1cs* R, const Fr* d_
     const CsrMatrix M{(const uint32_t*)R->d_off, (const uint32_t*)R->d_idx, (const Fr*)R->d_coef, (const uint32_t*)R->d_rows,
                       R->n_short, R->n_warp, R->n_cta, (uint32_t)R->n};
     return csr_eval_queue(ctx, st, M, d_in, (uint32_t)R->n_inputs, d_aux, oa, ob, oc);
+}
+
+// bb_r1cs_check(_batch) after the argument checks: `count` witnesses (row-major, bb_groth16_prove_r1cs_batch's layout)
+// checked item by item on the main stream through one a, b, c block and, for host witnesses, one upload block.  The
+// per-item first rows and counts stay on the device until one download at the end; bits (count = 1 only) likewise.
+int r1cs_check_run(bb_ctx* ctx, const bb_r1cs* R, const void* inputs, const void* aux, size_t count, int on_device, size_t* first,
+                   size_t* n_unsat, uint64_t* bits) {
+    BB_CUDA(cudaSetDevice(ctx->device));
+    NvtxRange nvtx("r1cs_check");
+    cudaStream_t st = ctx->main_stream;
+    const size_t n = R->n, ni = R->n_inputs, na = R->n_aux, words = (n + 63) / 64;
+    DevBuf d_abc, d_res, d_bits, up[2];
+    BB_TRY(d_abc.alloc(ctx, 3 * n * 32));
+    BB_TRY(d_res.alloc(ctx, 2 * count * 4));                     // first[count], then n_unsat[count]
+    uint32_t *r_first = d_res.as<uint32_t>(), *r_count = r_first + count;
+    BB_CUDA(cudaMemsetAsync(r_first, 0xFF, count * 4, st));
+    BB_CUDA(cudaMemsetAsync(r_count, 0, count * 4, st));
+    if (bits) {
+        BB_TRY(d_bits.alloc(ctx, words * 8));
+        BB_CUDA(cudaMemsetAsync(d_bits.p, 0, words * 8, st));
+    }
+    if (!on_device) {
+        BB_TRY(up[0].alloc(ctx, ni * 32));
+        BB_TRY(up[1].alloc(ctx, na * 32));
+    }
+    Fr* oa = d_abc.as<Fr>();
+    StageTimer tm(ctx, st);
+    tm.mark("r1cs_check.begin");
+    for (size_t i = 0; i < count; i++) {
+        const char* in_i = (const char*)inputs + i * ni * 32;
+        const char* aux_i = na ? (const char*)aux + i * na * 32 : nullptr;
+        const Fr *d_in = (const Fr*)in_i, *d_aux = (const Fr*)aux_i;
+        if (!on_device) {                                          // the stream orders this copy after item i - 1's reads
+            BB_CUDA(cudaMemcpyAsync(up[0].p, in_i, ni * 32, cudaMemcpyHostToDevice, st));
+            if (na) BB_CUDA(cudaMemcpyAsync(up[1].p, aux_i, na * 32, cudaMemcpyHostToDevice, st));
+            ctx->h2d_bytes += (ni + na) * 32;
+            d_in = up[0].as<Fr>();
+            d_aux = up[1].as<Fr>();
+        }
+        tm.mark("r1cs_check.upload");
+        BB_TRY(r1cs_eval_queue(ctx, st, R, d_in, d_aux, oa, oa + n, oa + 2 * n));
+        tm.mark("r1cs_check.eval");
+        k_r1cs_check<<<cdiv(n, 256), 256, 0, st>>>(oa, oa + n, oa + 2 * n, (uint32_t)n, r_first + i, r_count + i, d_bits.as<uint32_t>());
+        ctx->count_launch();
+        BB_CUDA(cudaGetLastError());
+        tm.mark("r1cs_check.compare");
+    }
+    std::vector<uint32_t> res(2 * count);
+    BB_CUDA(cudaMemcpyAsync(res.data(), r_first, 2 * count * 4, cudaMemcpyDeviceToHost, st));
+    if (bits) BB_CUDA(cudaMemcpyAsync(bits, d_bits.p, words * 8, cudaMemcpyDeviceToHost, st));
+    ctx->d2h_bytes += 2 * count * 4 + (bits ? words * 8 : 0);
+    BB_CUDA(cudaStreamSynchronize(st));
+    tm.report(R->nnz[0] + R->nnz[1] + R->nnz[2]);
+    for (size_t i = 0; i < count; i++) {
+        first[i] = res[i] == 0xFFFFFFFFu ? SIZE_MAX : res[i];
+        if (n_unsat) n_unsat[i] = res[count + i];
+    }
+    return BB_OK;
 }
 
 }  // namespace
@@ -366,6 +437,22 @@ int bb_groth16_prove_r1cs_batch(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* R
         return BB_OK;
     };
     return prove_batch_impl(ctx, crs, ws.data(), count, r, s, proofs, status, &fill);
+}
+
+int bb_r1cs_check(bb_ctx* ctx, const bb_r1cs* R, const void* input, size_t n_inputs, const void* aux, size_t n_aux, int on_device,
+                  size_t* first, size_t* count, uint64_t* unsat_bits) {
+    if (!ctx || !R || !first || !count) { set_error("bb_r1cs_check: null argument"); return BB_ERR_ARG; }
+    BB_TRY(check_witness("bb_r1cs_check", ctx, R, input, n_inputs, aux, n_aux, on_device, true));
+    return r1cs_check_run(ctx, R, input, aux, 1, on_device, first, count, unsat_bits);
+}
+
+int bb_r1cs_check_batch(bb_ctx* ctx, const bb_r1cs* R, const void* inputs, size_t n_inputs, const void* aux, size_t n_aux, size_t count,
+                        int on_device, size_t* first, size_t* n_unsat) {
+    if (!ctx || !R) { set_error("bb_r1cs_check_batch: null argument"); return BB_ERR_ARG; }
+    if (!count) return BB_OK;
+    if (!first) { set_error("bb_r1cs_check_batch: null argument"); return BB_ERR_ARG; }
+    BB_TRY(check_witness("bb_r1cs_check_batch", ctx, R, inputs, n_inputs, aux, n_aux, on_device, true));
+    return r1cs_check_run(ctx, R, inputs, aux, count, on_device, first, n_unsat, nullptr);
 }
 
 }  // extern "C"

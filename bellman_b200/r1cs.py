@@ -96,12 +96,7 @@ class R1CS(_DeviceObject):
     @classmethod
     def synth_mimc(cls, worker, rounds, seed):
         """bench-only: the MiMC circuit of bb_synth_mimc_witness(rounds, seed) (same constants), from bb_synth_mimc_r1cs"""
-        mats = []
-        for terms in (3 * rounds, 4 * rounds, 3 * rounds):
-            mats.append((np.zeros(2 * rounds + 1, np.uint64), np.zeros(terms, np.uint32), np.zeros((terms, 4), np.uint64)))
-        args = [_ptr(x) for m in mats for x in m]
-        _check(load_library().bb_synth_mimc_r1cs(C.c_size_t(rounds), C.c_uint64(seed), *args))
-        return cls(worker, 2, 2 * rounds + 1, *mats)
+        return cls(worker, 2, 2 * rounds + 1, *synth_mimc_matrices(rounds, seed))
 
     def density_words(self):
         """(a_aux_density, b_input_density, b_aux_density) as bb_witness's LSB-first uint64 words"""
@@ -130,6 +125,27 @@ class R1CS(_DeviceObject):
         del keep
         return None if res is None else tuple(res)
 
+    def unsatisfied(self, input_assignment, aux_assignment, on_device=False, bits=False):
+        """bb_r1cs_check: (first, count) -- the lowest row k with <A_k,z> <B_k,z> != <C_k,z> (None if every row holds) and
+        how many rows fail; with bits=True also a bool array of n_constraints marking them.  Rows are numbered as eval's
+        outputs (the appended input rows never fail).  Witness arguments as eval's."""
+        src, keep = self._witness_args(input_assignment, aux_assignment, on_device)
+        first, count = C.c_size_t(), C.c_size_t()
+        words = np.zeros((self.n_constraints + 63) // 64, np.uint64) if bits else None
+        _check(load_library().bb_r1cs_check(self.worker._h, self._h, *src, C.byref(first), C.byref(count), _ptr(words)))
+        del keep
+        res = (_first_or_none(first.value), count.value)
+        return res + (_unpack(words, self.n_constraints),) if bits else res
+
+    def which_is_unsatisfied(self, input_assignment, aux_assignment, on_device=False):
+        """TestConstraintSystem::which_is_unsatisfied (src/gadgets/test/mod.rs:254-267) on the device: the index of the
+        first failing constraint, or None (constraints have no names here)"""
+        return self.unsatisfied(input_assignment, aux_assignment, on_device)[0]
+
+    def is_satisfied(self, input_assignment, aux_assignment, on_device=False):
+        """TestConstraintSystem::is_satisfied (src/gadgets/test/mod.rs:269-272) on the device"""
+        return self.which_is_unsatisfied(input_assignment, aux_assignment, on_device) is None
+
     def _witness_args(self, input_assignment, aux_assignment, on_device):
         """the (input, n_inputs, aux, n_aux, on_device) arguments of bb_r1cs_eval and bb_groth16_prove_r1cs, and the host
         arrays they point into: device addresses (lengths taken from the constraint system), or host arrays"""
@@ -148,6 +164,49 @@ class R1CS(_DeviceObject):
         asg.input_assignment, asg.aux_assignment = _c64(input_assignment, 4), _c64(aux_assignment, 4)
         asg.a_aux_density, asg.b_input_density, asg.b_aux_density = self.density_words()
         return asg
+
+
+def synth_mimc_matrices(rounds, seed):
+    """bench-only: the A, B, C matrices of bb_synth_mimc_r1cs(rounds, seed), (row_offsets, vars, coeffs) each, as
+    R1CS.synth_mimc uploads them (2 inputs, 2 rounds + 1 aux, 2 rounds constraints before the input rows)"""
+    mats = []
+    for terms in (3 * rounds, 4 * rounds, 3 * rounds):
+        mats.append((np.zeros(2 * rounds + 1, np.uint64), np.zeros(terms, np.uint32), np.zeros((terms, 4), np.uint64)))
+    args = [_ptr(x) for m in mats for x in m]
+    _check(load_library().bb_synth_mimc_r1cs(C.c_size_t(rounds), C.c_uint64(seed), *args))
+    return mats
+
+
+def _first_or_none(v):
+    return None if v == C.c_size_t(-1).value else int(v)
+
+
+def _batch_witness_args(r1cs, inputs, aux, count, device_ptrs):
+    """the (inputs, n_inputs, aux, n_aux, count, on_device) arguments of bb_r1cs_check_batch, and the host arrays they point
+    into (count = 0: null pointers, nothing to read)"""
+    if device_ptrs is not None or not count:
+        d = device_ptrs or {"inputs": None, "aux": None}
+        return (C.c_void_p(_addr(d["inputs"])), C.c_size_t(r1cs.n_inputs), C.c_void_p(_addr(d["aux"])),
+                C.c_size_t(r1cs.n_aux), C.c_size_t(count), C.c_int(device_ptrs is not None)), ()
+    inp = np.ascontiguousarray(np.asarray(inputs, dtype=np.uint64).reshape(count, -1, 4))
+    ax = np.ascontiguousarray(np.asarray(aux, dtype=np.uint64).reshape(count, -1, 4))
+    return (_ptr(inp), C.c_size_t(inp.shape[1]), _ptr(ax), C.c_size_t(ax.shape[1]), C.c_size_t(count), C.c_int(0)), (inp, ax)
+
+
+def check_r1cs_batch(r1cs, inputs, aux, count=None, device_ptrs=None):
+    """bb_r1cs_check_batch: R1CS.unsatisfied for `count` witnesses in one call (count defaults to len(inputs); with
+    device_ptrs it must be given).  inputs / aux / device_ptrs as create_proof_r1cs_batch takes them.  Returns one
+    (first or None, count) per item."""
+    if count is None:
+        if device_ptrs is not None:
+            raise ValueError("check_r1cs_batch: count is required with device_ptrs")
+        count = len(inputs)
+    src, keep = _batch_witness_args(r1cs, inputs, aux, count, device_ptrs)
+    first = np.zeros(max(count, 1), np.uint64)
+    n_unsat = np.zeros(max(count, 1), np.uint64)
+    _check(load_library().bb_r1cs_check_batch(r1cs.worker._h, r1cs._h, *src, _ptr(first), _ptr(n_unsat)))
+    del keep
+    return [(_first_or_none(int(f)), int(k)) for f, k in zip(first[:count], n_unsat[:count])]
 
 
 def create_proof_r1cs(r1cs, params, input_assignment, aux_assignment, r, s, device_ptrs=None):

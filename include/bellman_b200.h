@@ -89,8 +89,8 @@ void bb_ctx_destroy(bb_ctx* ctx);
  *   params_read_chunk  bb_params_read / bb_vk_read from host memory: staging bytes per chunk (default 64 MiB; rounded
  *                      down to whole points, at least one point)
  *   ntt_tile_log, ntt_col_bits   shape of the NTT tiles
- *   profile            1 = CUDA-event timing of the MSM stages, and of the verify.*, decode.*, r1cs.*, params.* and
- *                      generate.* stages (bb_profile_read)
+ *   profile            1 = CUDA-event timing of the MSM stages, and of the verify.*, decode.*, r1cs.*, r1cs_check.*,
+ *                      params.* and generate.* stages (bb_profile_read)
  *   msm_acc_variant, msm_affine_tma, msm_reduce_2d, ntt_radix8   retired: accepted for compatibility, no effect */
 int bb_ctx_set_option(bb_ctx* ctx, const char* key, long value);
 int bb_ctx_synchronize(bb_ctx* ctx);
@@ -339,6 +339,18 @@ int bb_groth16_prove_r1cs(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* r1cs, c
 int bb_groth16_prove_r1cs_batch(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* r1cs, const void* inputs, size_t n_inputs,
                                 const void* aux, size_t n_aux, size_t count, int on_device, const uint8_t* r, const uint8_t* s,
                                 uint8_t* proofs, int* status);
+/* TestConstraintSystem::which_is_unsatisfied / is_satisfied (src/gadgets/test/mod.rs:254-272) over the resident constraint
+ * system: *first = the lowest row k with <A_k,z> <B_k,z> != <C_k,z> (SIZE_MAX if none), *count = the number of such rows,
+ * unsat_bits (may be NULL; host; (n + 63) / 64 words, n = bb_r1cs_info shape[0]) = those rows as LSB-first bits.  Rows are
+ * numbered as bb_r1cs_eval's outputs; the appended input rows never fail.  Input 0 is taken as given.  Argument errors
+ * exactly bb_r1cs_eval's (check_witness), before any device work.  Blocking. */
+int bb_r1cs_check(bb_ctx* ctx, const bb_r1cs* r1cs, const void* input, size_t n_inputs, const void* aux, size_t n_aux,
+                  int on_device, size_t* first, size_t* count, uint64_t* unsat_bits);
+/* the same for `count` witnesses laid out as bb_groth16_prove_r1cs_batch's; first[i] / n_unsat[i] (n_unsat may be NULL) are
+ * bb_r1cs_check's for item i alone.  count = 0: BB_OK, nothing written.  The items run one after another through one
+ * a, b, c block (and one upload block for host witnesses): device memory is that of one witness whatever the count. */
+int bb_r1cs_check_batch(bb_ctx* ctx, const bb_r1cs* r1cs, const void* inputs, size_t n_inputs, const void* aux, size_t n_aux,
+                        size_t count, int on_device, size_t* first, size_t* n_unsat);
 
 /* ---- generating keys: generate_parameters / generate_random_parameters (groth16/src/generator.rs:21-40,159-507) ----------
  * The key of a resident constraint system, computed on the device, element for element the reference's: the rows are the

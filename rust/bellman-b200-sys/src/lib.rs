@@ -216,6 +216,10 @@ extern "C" {
     pub fn bb_groth16_prove_r1cs_batch(ctx: *mut bb_ctx, crs: *const bb_crs, r1cs: *const bb_r1cs, inputs: *const c_void,
                                        n_inputs: usize, aux: *const c_void, n_aux: usize, count: usize, on_device: c_int,
                                        r: *const u8, s: *const u8, proofs: *mut u8, status: *mut c_int) -> c_int;
+    pub fn bb_r1cs_check(ctx: *mut bb_ctx, r1cs: *const bb_r1cs, input: *const c_void, n_inputs: usize, aux: *const c_void,
+                         n_aux: usize, on_device: c_int, first: *mut usize, count: *mut usize, unsat_bits: *mut u64) -> c_int;
+    pub fn bb_r1cs_check_batch(ctx: *mut bb_ctx, r1cs: *const bb_r1cs, inputs: *const c_void, n_inputs: usize, aux: *const c_void,
+                               n_aux: usize, count: usize, on_device: c_int, first: *mut usize, n_unsat: *mut usize) -> c_int;
 
     pub fn bb_vk_prepare(ctx: *mut bb_ctx, desc: *const bb_vk_desc, out: *mut *mut bb_vk) -> c_int;
     pub fn bb_vk_destroy(vk: *mut bb_vk);

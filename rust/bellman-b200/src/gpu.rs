@@ -346,6 +346,23 @@ impl GpuR1cs {
         status(unsafe { bb_r1cs_create(worker.ctx, &desc, &mut handle) })?;
         Ok(GpuR1cs { ctx: worker.ctx, handle, n_inputs: ni, n_aux: na })
     }
+
+    /// `TestConstraintSystem::which_is_unsatisfied` (src/gadgets/test/mod.rs:254-267) on the device (bb_r1cs_check): the
+    /// index of the first constraint with <A_k,z> <B_k,z> != <C_k,z> for the witness `WitnessCS` collects (input 0 = ONE
+    /// included), or None.  Constraints have no names here; the index is the enforce order.
+    pub fn which_is_unsatisfied(&self, input_assignment: &[Scalar], aux_assignment: &[Scalar]) -> Result<Option<usize>, SynthesisError> {
+        let (mut first, mut count) = (0usize, 0usize);
+        status(unsafe {
+            bb_r1cs_check(self.ctx, self.handle, input_assignment.as_ptr() as _, input_assignment.len(), aux_assignment.as_ptr() as _,
+                          aux_assignment.len(), 0, &mut first, &mut count, ptr::null_mut())
+        })?;
+        Ok(if first == usize::MAX { None } else { Some(first) })
+    }
+
+    /// `TestConstraintSystem::is_satisfied` (src/gadgets/test/mod.rs:269-272) on the device
+    pub fn is_satisfied(&self, input_assignment: &[Scalar], aux_assignment: &[Scalar]) -> Result<bool, SynthesisError> {
+        Ok(self.which_is_unsatisfied(input_assignment, aux_assignment)?.is_none())
+    }
 }
 impl Drop for GpuR1cs {
     fn drop(&mut self) { unsafe { bb_r1cs_destroy(self.handle) } }
