@@ -13,7 +13,8 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 CSRC = os.path.join(ROOT, "bellman_b200", "csrc")
-SOURCES = ["capi.cu", "ntt.cu", "msm.cu", "prover.cu", "synth.cu"]
+# the translation units libbellman_b200.so links, in the Makefile's order
+SOURCES = re.search(r"^SRCS\s*:=(.*)$", open(os.path.join(CSRC, "Makefile")).read(), re.M).group(1).split()
 
 _KERNEL = re.compile(r"([A-Za-z_]\w*(?:<[^<>();]*>)?)<<<")
 
@@ -101,7 +102,7 @@ def build(out_dir, extra_flags=(), emulate_ptx=True):
         obj = cpp.replace(".cpp", ".o")
         cmd = ["g++", "-O2", "-std=c++20", "-fPIC", "-pthread", "-w", *(["-DBB_EMULATE_PTX"] if emulate_ptx else []), *extra_flags,
                "-I", os.path.join(ROOT, "tests", "native", "cuda_emu"), "-I", CSRC, "-c", cpp, "-o", obj]
-        procs.append((cmd, subprocess.Popen(cmd)))          # the five translation units compile side by side
+        procs.append((cmd, subprocess.Popen(cmd)))          # the translation units compile side by side
         objs.append(obj)
     for cmd, proc in procs:
         if proc.wait() != 0:

@@ -6,7 +6,8 @@ import os
 import subprocess
 import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from emulated import ROOT, bench_dry_run, dry_run_script
+
 REQUIRED = {"impl", "metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better",
             "scaling", "vs_baseline", "dtype", "data", "config", "cpu_baseline", "e2e"}
 
@@ -41,38 +42,14 @@ def test_reference_arm_under_torchrun_world2():
     _check_line(res.stdout, 2)
 
 
-DRY_RUN = '''
-import importlib.util, sys
-sys.path.insert(0, ROOT)
-import torch
-torch.cuda.set_device = lambda *a, **k: None
-torch.cuda.synchronize = lambda *a, **k: None
-_to = torch.Tensor.to
-torch.Tensor.to = lambda self, *a, **k: self if (a and isinstance(a[0], str) and a[0].startswith("cuda")) else _to(self, *a, **k)
-torch.Tensor.pin_memory = lambda self, *a, **k: self
-import bellman_b200 as bb
-bb.LIB_PATH, bb._lib = EMU_LIB, None          # the product sources on host fibers (tests/native)
-import os
-os.environ["LOCAL_RANK"] = "0"                # the emulation has one device: under torchrun every rank uses it
-spec = importlib.util.spec_from_file_location("bench", ROOT + "/bench.py")
-bench = importlib.util.module_from_spec(spec)
-spec.loader.exec_module(bench)
-sys.argv = ["bench.py", "--log-size", "8", "--steps", "2", "--warmup", "1", "--cpu-sample-log", "8", "--autotune-reps", "1", "--autotune", "2"] + EXTRA
-bench.main()
-'''
+ARGV = ["--log-size", "8", "--steps", "2", "--warmup", "1", "--cpu-sample-log", "8", "--autotune-reps", "1", "--autotune", "2"]
 
 
 def test_own_arm_dry_run_on_the_emulated_device(tmp_path, emu_lib):
     """bench.py's default workload (prove: value leg, e2e leg, roofline, timeline, cpu_baseline) end
     to end with the CUDA library replaced by the host-fiber build of the same sources and torch.cuda
     stubbed: checks the script and the JSON contract, not the numbers."""
-    script = tmp_path / "dry.py"
-    script.write_text(f"ROOT = {ROOT!r}\nEMU_LIB = {emu_lib!r}\nEXTRA = []\n" + DRY_RUN)
-    res = subprocess.run([sys.executable, str(script)], capture_output=True, text=True, timeout=900, cwd=ROOT)
-    assert res.returncode == 0, res.stderr[-3000:]
-    lines = [l for l in res.stdout.splitlines() if l.strip()]
-    assert len(lines) == 1, res.stdout
-    d = json.loads(lines[0])
+    d = bench_dry_run(emu_lib, tmp_path, "bench.py", ARGV)
     need = {"metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline",
             "dtype", "data", "config", "e2e", "gpu_launches", "clocks", "roofline", "cpu_baseline", "timeline"}
     assert need <= set(d), need - set(d)
@@ -93,18 +70,11 @@ def test_tuner_child_mode_and_parent_fallback(tmp_path, emu_lib):
     container) records the error and measures the default form."""
     # (the unsharded tuner itself runs in the dry run above; here) the child of rank 1 of 2 -- the gate in front of the
     # collective tuner: that rank's key shard, no process group
-    script = tmp_path / "child_shard.py"
-    script.write_text(f"ROOT = {ROOT!r}\nEMU_LIB = {emu_lib!r}\nEXTRA = ['--tune-child', '--shard-index', '1', '--shard-count', '2']\n" + DRY_RUN)
     env = dict(os.environ, WORLD_SIZE="2", RANK="1", LOCAL_RANK="0")
-    res = subprocess.run([sys.executable, str(script)], capture_output=True, text=True, timeout=900, cwd=ROOT, env=env)
-    assert res.returncode == 0, res.stderr[-3000:]
-    rep = json.loads([l for l in res.stdout.splitlines() if l.strip()][-1])["tune_child"]
+    rep = bench_dry_run(emu_lib, tmp_path, "bench.py", ARGV + ["--tune-child", "--shard-index", "1", "--shard-count", "2"],
+                        env=env)["tune_child"]
     assert all(t > 0 for t in rep["ms"]) and rep["name"]
-    script = tmp_path / "parent.py"
-    script.write_text(f"ROOT = {ROOT!r}\nEMU_LIB = {emu_lib!r}\nEXTRA = ['--autotune', '1', '--no-cpu-baseline']\n" + DRY_RUN)
-    res = subprocess.run([sys.executable, str(script)], capture_output=True, text=True, timeout=900, cwd=ROOT)
-    assert res.returncode == 0, res.stderr[-3000:]
-    d = json.loads([l for l in res.stdout.splitlines() if l.strip()][-1])
+    d = bench_dry_run(emu_lib, tmp_path, "bench.py", ARGV + ["--autotune", "1", "--no-cpu-baseline"])
     at = d["autotune"]
     assert at["error"] and at["chosen"] == 0 and at["where"] == "child process" and "tuner process failed" in d["config"]["msm_form"]
     assert d["value"] > 0 and d["gpu_launches"] > 100
@@ -114,8 +84,7 @@ def test_own_arm_dry_run_two_ranks(tmp_path, emu_lib):
     """bench.py --gpus 2 under torchrun with gloo and the emulated device: the sharded step, the max over ranks, the gate in
     front of the collective tuner (the per-rank tuner children cannot run here -- no CUDA device -- so both ranks must stay on
     the default form and say why), the sharded proof == single-GPU proof check, one JSON line from rank 0."""
-    script = tmp_path / "dry2.py"
-    script.write_text(f"ROOT = {ROOT!r}\nEMU_LIB = {emu_lib!r}\nEXTRA = ['--gpus', '2', '--autotune', '1', '--no-cpu-baseline']\n" + DRY_RUN)
+    script = dry_run_script(emu_lib, tmp_path, "bench.py", ARGV + ["--gpus", "2", "--autotune", "1", "--no-cpu-baseline"])
     env = dict(os.environ, BB_BENCH_DIST_BACKEND="gloo")
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",
            "--master-port", "29541", str(script)]
@@ -134,11 +103,7 @@ def test_own_arm_dry_run_two_ranks(tmp_path, emu_lib):
 def test_msm_microbench_dry_run_on_the_emulated_device(tmp_path, emu_lib):
     """bench.py --workload msm (BASELINE configs[2] shape, here 2^10 points): both MSM forms are measured, the result
     is asserted against [sum k_i e_i]G inside the script"""
-    script = tmp_path / "dry_msm.py"
-    script.write_text(f"ROOT = {ROOT!r}\nEMU_LIB = {emu_lib!r}\nEXTRA = ['--workload', 'msm', '--log-size', '10']\n" + DRY_RUN)
-    res = subprocess.run([sys.executable, str(script)], capture_output=True, text=True, timeout=900, cwd=ROOT)
-    assert res.returncode == 0, res.stderr[-3000:]
-    d = json.loads([l for l in res.stdout.splitlines() if l.strip()][0])
+    d = bench_dry_run(emu_lib, tmp_path, "bench.py", ARGV + ["--workload", "msm", "--log-size", "10"])
     assert d["metric"] == "g1_msm_mpt_per_sec" and d["config"]["result_check"].endswith("equal")
     assert len(d["autotune"]["ms"]) == 2 and all(t > 0 for t in d["autotune"]["ms"])
 

@@ -20,21 +20,9 @@ import bellman_b200 as bb
 from oracle import o1
 
 import test_gpu_parity as G
+from emulated import ROOT, use_library, worker  # noqa: F401  (the emulated-library fixture)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 R = o1.FR_MODULUS
-
-
-@pytest.fixture(scope="module")
-def worker(emu_lib):
-    saved = (bb.LIB_PATH, bb._lib)
-    bb.LIB_PATH, bb._lib = emu_lib, None             # this module only: the mirror talks to the emulated library
-    try:
-        w = bb.Worker(0)
-        yield w
-        w.close()
-    finally:
-        bb.LIB_PATH, bb._lib = saved
 
 
 def test_emulated_field_and_point_kernels(worker):
@@ -290,9 +278,7 @@ def test_emulated_pipeline_over_the_host_arithmetic_path(tmp_path):
     be = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(be)
     lib, _ = be.build(str(tmp_path / "emu_host"), emulate_ptx=False)
-    saved = (bb.LIB_PATH, bb._lib)
-    bb.LIB_PATH, bb._lib = lib, None
-    try:
+    with use_library(lib):
         w = bb.Worker(0)
         G.test_field_arithmetic(w)
         G.test_point_arithmetic(w)
@@ -306,8 +292,6 @@ def test_emulated_pipeline_over_the_host_arithmetic_path(tmp_path):
         r, s = rng.randrange(R), rng.randrange(R)
         assert bb.create_proof(G._assignment(mc.witness()), bb.Parameters(w, mc.export_params()), r, s) == mc.prove(r, s)
         w.close()
-    finally:
-        bb.LIB_PATH, bb._lib = saved
 
 
 def test_emulated_prove_begin_end(worker):

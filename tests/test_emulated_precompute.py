@@ -9,7 +9,7 @@ from oracle import o1
 
 import test_gpu_parity as G
 import test_emulated_pipeline as E
-from test_emulated_pipeline import worker                       # noqa: F401  (the emulated-library fixture)
+from emulated import worker  # noqa: F401  (the emulated-library fixture)
 
 
 @pytest.fixture()

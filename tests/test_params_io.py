@@ -7,26 +7,14 @@ import struct
 import numpy as np
 import pytest
 
-import bellman_b200 as bb
 from bellman_b200 import params_io
 from oracle import o1
 from oracle.oracle0 import fields as F
 
+from emulated import worker  # noqa: F401  (the curve / subgroup checks are device code: they run on the emulated library)
+
 R = o1.FR_MODULUS
 P = o1.FP_MODULUS
-
-
-@pytest.fixture(scope="module")
-def worker(emu_lib):
-    """the curve / subgroup checks are device code: here they run in the host-fiber build of the sources"""
-    saved = (bb.LIB_PATH, bb._lib)
-    bb.LIB_PATH, bb._lib = emu_lib, None
-    try:
-        w = bb.Worker(0)
-        yield w
-        w.close()
-    finally:
-        bb.LIB_PATH, bb._lib = saved
 
 
 def _params(sizes, seed=1):
