@@ -195,6 +195,24 @@ __global__ void k_selftest_fp_inv(const Fp* a, Fp* o, size_t n, int op) {
     Fp x = a[i];
     o[i] = x.is_zero() ? x : (op == 4 ? fp_inv_gcd(x) : fp_inv(x));
 }
+// Fp2: op 0 operator* and 3 sqr() (the out-of-line calls of the tower and the verifier), 1 +, 2 -, 4 fp2_inv (zero -> zero),
+// 5 mul_inl and 6 sqr_inl (the inlined forms of the halving rounds)
+__global__ void k_selftest_fp2(const Fp2* a, const Fp2* b, Fp2* o, size_t n, int op) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    Fp2 x = a[i], y = b[i];
+    Fp2 r;
+    switch (op) {
+        case 0: r = x * y; break;
+        case 1: r = x + y; break;
+        case 2: r = x - y; break;
+        case 3: r = x.sqr(); break;
+        case 4: r = x.is_zero() ? x : fp2_inv(x); break;
+        case 5: r = x.mul_inl(y); break;
+        default: r = x.sqr_inl(); break;
+    }
+    o[i] = r;
+}
 template <class F>
 __global__ void k_selftest_point(const Affine<F>* a, const Affine<F>* b, Affine<F>* o, size_t n, int op) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -617,6 +635,7 @@ int bb_selftest_field(bb_ctx* ctx, int field, int op, const void* a, const void*
         return BB_OK;
     }
     if (field == 1) return selftest_run<Fp>(ctx, k_selftest_field<Fp>, a, b, out, n, op);
+    if (field == 2 && op >= 0 && op <= 6) return selftest_run<Fp2>(ctx, k_selftest_fp2, a, b, out, n, op);
     return BB_ERR_ARG;
 }
 int bb_selftest_point(bb_ctx* ctx, int group, int op, const void* a, const void* b, void* out, size_t n) {

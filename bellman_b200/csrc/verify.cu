@@ -127,7 +127,8 @@ __global__ void k_final_exp(const Fp12* __restrict__ f, Fp12* gt, uint32_t* verd
     *verdict = r.is_one() ? 1u : 0u;
 }
 
-// diagnostics: element-wise tower operations (bb_diag_fp12)
+// diagnostics: element-wise tower operations (bb_diag_fp12).  The inverse and the final exponentiation map zero to zero,
+// as k_final_exp does: both invert, and the binary Euclidean inversion does not terminate on zero.
 __global__ void __launch_bounds__(64) k_diag_fp12(const Fp12* __restrict__ a, const Fp12* __restrict__ b, size_t n, int op, Fp12* out) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -136,11 +137,11 @@ __global__ void __launch_bounds__(64) k_diag_fp12(const Fp12* __restrict__ a, co
     switch (op) {
         case 0: r = fp12_mul(x, y); break;
         case 1: r = fp12_sqr(x); break;
-        case 2: r = fp12_inv(x); break;
+        case 2: r = x.is_zero() ? x : fp12_inv(x); break;
         case 3: r = fp12_cyclotomic_sqr(x); break;
         case 4: r = fp12_frob1(x); break;
         case 5: r = fp12_frob2(x); break;
-        case 6: r = fp12_final_exp(x); break;
+        case 6: r = x.is_zero() ? x : fp12_final_exp(x); break;
         default: r = fp12_mul_line(x, y.c0.c0, y.c0.c1, y.c1.c1); break;
     }
     out[i] = r;

@@ -36,7 +36,9 @@ int bb_synth_mimc_r1cs(size_t rounds, uint64_t seed, uint64_t* a_off, uint32_t* 
 
 /* ---- diagnostics (used by the parity tests; not part of the bellman-facing surface) ------ */
 /* element-wise on the device: field 0 = Fr, 1 = Fp (Montgomery); op 0 mul, 1 add, 2 sub, 3 sqr;
- * Fp only: 4 = inverse by the binary Euclidean algorithm (fp_inv_gcd), 5 = inverse as a^(p-2); 0 -> 0 */
+ * Fp only: 4 = inverse by the binary Euclidean algorithm (fp_inv_gcd), 5 = inverse as a^(p-2); 0 -> 0.
+ * field 2 = Fp2, elements 24 u64 (c0 then c1, Montgomery): op 0 mul (the out-of-line operator*), 1 add, 2 sub,
+ * 3 sqr (the out-of-line sqr()), 4 inverse (fp2_inv; 0 -> 0), 5 mul_inl, 6 sqr_inl (the inlined forms) */
 int bb_selftest_field(bb_ctx* ctx, int field, int op, const void* a, const void* b, void* out, size_t n);
 /* element-wise on affine points: op 0: a + b (mixed add); 1: 2a + b; 2: a + (2b - b) */
 int bb_selftest_point(bb_ctx* ctx, int group, int op, const void* a, const void* b, void* out, size_t n);
@@ -56,7 +58,8 @@ int bb_diag_multi_pairing(bb_ctx* ctx, size_t n, const void* g1, const void* g2,
 /* k of the G_T convention: bb_diag_multi_pairing returns e(P, Q)^k for the pairing e = f_{|x|,Q}(P)^((p^12 - 1) / r) */
 int bb_diag_gt_exponent(void);
 /* element-wise on n Fp12 values (12 Montgomery Fp each, tower order): op 0 a*b, 1 a^2, 2 1/a, 3 cyclotomic squaring of a,
- * 4 a^p, 5 a^(p^2), 6 the final exponentiation a^(3 (p^12 - 1) / r), 7 a times the sparse line (b.c0.c0 + b.c0.c1 v) + (b.c1.c1 v) w */
+ * 4 a^p, 5 a^(p^2), 6 the final exponentiation a^(3 (p^12 - 1) / r), 7 a times the sparse line (b.c0.c0 + b.c0.c1 v) + (b.c1.c1 v) w;
+ * ops 2 and 6 map zero to zero */
 int bb_diag_fp12(bb_ctx* ctx, int op, const void* a, const void* b, void* out, size_t n);
 /* bb_groth16_verify_batch, also writing the G_T value its verdict was taken from (format of bb_diag_multi_pairing) */
 int bb_diag_verify_batch_gt(bb_ctx* ctx, const bb_vk* vk, const bb_proof_batch* batch, const void* z, void* gt_out);
