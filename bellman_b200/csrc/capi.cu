@@ -1,5 +1,6 @@
 // bellman_b200: C-ABI entry points that are not MSM / prover specific (include/bellman_b200.h).
 #include "bb_internal.cuh"
+#include "encoding.cuh"
 #include "fixed_table.cuh"
 
 using namespace bb;
@@ -12,8 +13,6 @@ void set_error(const char* fmt, ...) {
     vsnprintf(g_err, sizeof g_err, fmt, ap);
     va_end(ap);
 }
-void g1_compress(const G1Affine& p, uint8_t* out);
-void g2_compress(const G2Affine& p, uint8_t* out);
 G1X g1_host_mul(const G1X& p, const uint32_t* k);
 G2X g2_host_mul(const G2X& p, const uint32_t* k);
 }  // namespace bb
@@ -163,21 +162,15 @@ int fixed_base_mul(bb_ctx* ctx, FixedTable<F>& tab, const Affine<F>& gen, const 
 // beyond the encoding: y^2 = x^3 + b and [r]P = identity.  One thread per point; the first offending
 // index is reported through atomicMin (bad[0]: off the curve, bad[1]: outside the subgroup).  The
 // identity itself passes here: the callers decide where it is allowed.
-BB_HD Fp curve_b(const Fp*) { Fp four = Fp::zero(); four.l[0] = 4; return fp_from_canonical(four); }              // y^2 = x^3 + 4
-BB_HD Fp2 curve_b(const Fp2*) { Fp f = curve_b((const Fp*)nullptr); return {f, f}; }                               // y^2 = x^3 + 4(u + 1)
-
 template <class F>
 __global__ void __launch_bounds__(128) k_points_validate(const Affine<F>* __restrict__ pts, size_t n, int check_subgroup, uint32_t* bad) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     Affine<F> p = pts[i];
     if (p.is_identity()) return;
-    F lhs = p.y.sqr(), rhs = p.x.sqr() * p.x + curve_b((const F*)nullptr);
-    if (lhs != rhs) { atomicMin(&bad[0], (uint32_t)i); return; }
+    if (!on_curve(p)) { atomicMin(&bad[0], (uint32_t)i); return; }
     if (!check_subgroup) return;
-    const uint32_t r[8] = {BBC_FR_MOD_LIST};
-    XYZZ<F> q = XYZZ<F>::from_affine(p).mul_bits(r);
-    if (!q.is_identity()) atomicMin(&bad[1], (uint32_t)i);
+    if (!rP_is_identity(p)) atomicMin(&bad[1], (uint32_t)i);
 }
 
 // ---- diagnostics: element-wise field / point operations on the device ------------------------
@@ -553,8 +546,8 @@ int bb_point_mul(int group, const void* a, const void* k, int form, void* out) {
 }
 int bb_point_compress(int group, const void* a, uint8_t* out) {
     if (!a || !out) return BB_ERR_ARG;
-    if (group == BB_G1) { G1Affine p; std::memcpy(&p, a, 96); g1_compress(p, out); }
-    else if (group == BB_G2) { G2Affine p; std::memcpy(&p, a, 192); g2_compress(p, out); }
+    if (group == BB_G1) { G1Affine p; std::memcpy(&p, a, 96); encode_compressed(p, out); }
+    else if (group == BB_G2) { G2Affine p; std::memcpy(&p, a, 192); encode_compressed(p, out); }
     else return BB_ERR_ARG;
     return BB_OK;
 }
@@ -568,12 +561,7 @@ int bb_fp_convert(void* fp_inout, size_t n, int to_montgomery) {
         Fp x;
         std::memcpy(&x, v + i, sizeof x);
         if (to_montgomery) {
-            bool lt = false;                       // must be < p
-            for (int k = 11; k >= 0; k--) {
-                if (x.l[k] < bbc::FP_MOD[k]) { lt = true; break; }
-                if (x.l[k] > bbc::FP_MOD[k]) break;
-            }
-            if (!lt) { set_error("coordinate %zu is not a canonical field element", i); return BB_ERR_ARG; }
+            if (!is_canonical(x)) { set_error("coordinate %zu is not a canonical field element", i); return BB_ERR_ARG; }
             x = fp_from_canonical(x);
         } else {
             x = fp_to_canonical(x);

@@ -10,19 +10,12 @@
 //   5 identity        a valid encoding of the point at infinity (Proof::read: "point at infinity")
 // A proof reads A, then B, then C; its status is (which << 4) | why of the first failing element.
 //
-// Algorithms (variable time throughout: proof bytes are public data):
-//   Fp square root   a^((p+1)/4) (p = 3 mod 4) by a fixed 4-bit window over the constant exponent, then a squaring check
-//   Fp2 square root  Algorithm 9 of eprint 2012/685: a1 = a^((p-3)/4), alpha = a1^2 a, x0 = a1 a; x = u x0 if alpha = -1,
-//                    else (1 + alpha)^((p-1)/2) x0; then the squaring check
-//   subgroup, G1     phi(P) = -[x^2] P with phi(x, y) = (beta x, y)    (eprint 2021/1130; proof in 2022/352)
-//   subgroup, G2     psi(P) = [x] P with psi the untwist-Frobenius-twist map
-// x = -0xd201000000010000: [x^2] is two multiplications by |x| (126 doublings, 10 additions), [x] one.
+// The per-point rules, square roots and subgroup tests are encoding.cuh's.
 // Kernels (one thread per point):
 //   k_decode_g1      the 2n A and C points (or n packed points for the diagnostic)
 //   k_decode_g2      the n B points
 //   k_proof_status   folds the three element codes into the status byte, zeroes all points of an invalid proof
 //   k_encode_proofs  the inverse: Proof::write of n affine triples
-// Nothing outside this file calls into it.
 //
 // Parameters::read / VerifyingKey::read (groth16/src/lib.rs:158-218, 289-398) of a key file into a resident bb_crs / bb_vk:
 // the u32 length prefixes are walked on the host, every point is decoded on the device by
@@ -35,161 +28,13 @@
 #include <cstring>
 
 #include "bb_internal.cuh"
+#include "encoding.cuh"
 
 using namespace bb;
 
 namespace {
 
 constexpr unsigned DECODE_THREADS = 64;
-
-#if defined(__CUDACC__)
-static __device__ __constant__ uint32_t kExpSqrt[12] = {BBC_EXP_SQRT_LIST};     // (p + 1) / 4
-static __device__ __constant__ uint32_t kExpSqrt2[12] = {BBC_EXP_SQRT2_LIST};   // (p - 3) / 4
-static __device__ __constant__ uint32_t kFpHalf[12] = {BBC_FP_HALF_LIST};       // (p - 1) / 2
-#else
-static const uint32_t kExpSqrt[12] = {BBC_EXP_SQRT_LIST};
-static const uint32_t kExpSqrt2[12] = {BBC_EXP_SQRT2_LIST};
-static const uint32_t kFpHalf[12] = {BBC_FP_HALF_LIST};
-#endif
-
-constexpr int WHY_OK = 0, WHY_FLAGS = 1, WHY_NONCANONICAL = 2, WHY_NOT_ON_CURVE = 3, WHY_NOT_IN_SUBGROUP = 4, WHY_IDENTITY = 5;
-
-// a^e for a constant 384-bit exponent e (12 limbs), fixed 4-bit windows: 15 products for the table, then per window
-// four squarings and at most one product
-template <class F>
-BB_D F pow_fixed(const F& a, const uint32_t* e) {
-    F tab[16];
-    tab[0] = FieldOps<F>::one();
-    tab[1] = a;
-    for (int k = 2; k < 16; k++) tab[k] = tab[k - 1] * a;
-    int w = 95;
-    while (w > 0 && ((e[w >> 3] >> (4 * (w & 7))) & 15u) == 0) w--;
-    F r = tab[(e[w >> 3] >> (4 * (w & 7))) & 15u];
-    for (w--; w >= 0; w--) {
-        r = r.sqr(); r = r.sqr(); r = r.sqr(); r = r.sqr();
-        uint32_t d = (e[w >> 3] >> (4 * (w & 7))) & 15u;
-        if (d) r = r * tab[d];
-    }
-    return r;
-}
-
-template <class F> struct Root { F v; bool ok; };
-
-BB_D Root<Fp> fp_sqrt(const Fp& a) {
-    Fp r = pow_fixed(a, kExpSqrt);
-    return {r, r.sqr() == a};
-}
-
-BB_D Root<Fp2> fp2_sqrt(const Fp2& a) {
-    Fp2 a1 = pow_fixed(a, kExpSqrt2);
-    Fp2 alpha = a1.sqr() * a;
-    Fp2 x0 = a1 * a;
-    Fp2 minus_one{fp_one().neg(), Fp::zero()};
-    Fp2 x;
-    if (alpha == minus_one) x = Fp2{x0.c1.neg(), x0.c0};                            // u * x0
-    else x = pow_fixed(alpha + fp2_one(), kFpHalf) * x0;
-    return {x, x.sqr() == a};
-}
-
-BB_D Fp g1_b() { Fp four = Fp::zero(); four.l[0] = 4; return fp_from_canonical(four); }
-BB_D Fp2 g2_b() { Fp b = g1_b(); return {b, b}; }
-
-// 48 big-endian bytes -> canonical limbs; the top byte masked by mask0 (the flag bits)
-BB_D Fp fp_load_be(const uint8_t* s, uint32_t mask0) {
-    Fp r;
-    for (int k = 0; k < 12; k++) {
-        const uint8_t* q = s + 44 - 4 * k;
-        uint32_t b0 = k == 11 ? (q[0] & mask0) : q[0];
-        r.l[k] = (b0 << 24) | ((uint32_t)q[1] << 16) | ((uint32_t)q[2] << 8) | q[3];
-    }
-    return r;
-}
-BB_D void fp_store_be(const Fp& canonical, uint8_t* o) {
-    for (int k = 0; k < 12; k++) {
-        uint8_t* q = o + 44 - 4 * k;
-        uint32_t v = canonical.l[k];
-        q[0] = (uint8_t)(v >> 24); q[1] = (uint8_t)(v >> 16); q[2] = (uint8_t)(v >> 8); q[3] = (uint8_t)v;
-    }
-}
-BB_D bool fp_is_canonical(const Fp& x) {
-    for (int k = 11; k >= 0; k--) {
-        uint32_t m = Fp::modl(k);
-        if (x.l[k] != m) return x.l[k] < m;
-    }
-    return false;
-}
-// canonical y > (p - 1) / 2, for a Montgomery y
-BB_D bool fp_lexi_larger(const Fp& y) {
-    Fp c = fp_to_canonical(y);
-    for (int k = 11; k >= 0; k--)
-        if (c.l[k] != kFpHalf[k]) return c.l[k] > kFpHalf[k];
-    return false;
-}
-BB_D bool fp2_lexi_larger(const Fp2& y) { return y.c1.is_zero() ? fp_lexi_larger(y.c0) : fp_lexi_larger(y.c1); }
-BB_D Fp2 fp2_conj(const Fp2& a) { return {a.c0, a.c1.neg()}; }
-
-// [|x|] P, |x| = 0xd201000000010000: 63 doublings, 5 additions
-template <class F>
-BB_D XYZZ<F> mul_by_x_abs(const XYZZ<F>& p) {
-    XYZZ<F> acc = p;
-    for (int i = 62; i >= 0; i--) {
-        acc = acc.dbl();
-        if ((bbc::BLS_X_ABS >> i) & 1) acc.add(p);
-    }
-    return acc;
-}
-// q == (x, y) for an affine (x, y) that is not the identity
-template <class F>
-BB_D bool xyzz_equals_affine(const XYZZ<F>& q, const F& x, const F& y) {
-    return !q.is_identity() && q.X == x * q.ZZ && q.Y == y * q.ZZZ;
-}
-// phi(P) = -[x^2] P  <=>  [x^2] P = (beta x, -y)
-BB_D bool g1_in_subgroup(const G1Affine& p) {
-    G1X q = mul_by_x_abs(mul_by_x_abs(G1X::from_affine(p)));
-    return xyzz_equals_affine(q, p.x * Fp{{BBC_BETA_M_LIST}}, p.y.neg());
-}
-// psi(P) = [x] P = -[|x|] P  <=>  [|x|] P = -psi(P)
-BB_D bool g2_in_subgroup(const G2Affine& p) {
-    const Fp2 psi_x{Fp{{BBC_PSI_X_C0_M_LIST}}, Fp{{BBC_PSI_X_C1_M_LIST}}};
-    const Fp2 psi_y{Fp{{BBC_PSI_Y_C0_M_LIST}}, Fp{{BBC_PSI_Y_C1_M_LIST}}};
-    G2X q = mul_by_x_abs(G2X::from_affine(p));
-    return xyzz_equals_affine(q, fp2_conj(p.x) * psi_x, (fp2_conj(p.y) * psi_y).neg());
-}
-
-// from_compressed (check_subgroup != 0) or from_compressed_unchecked of one point; out = the point, or zeros unless 0
-template <class F> struct Decoded { Affine<F> p; int why; };
-
-BB_D Decoded<Fp> g1_decode(const uint8_t* s, bool check_subgroup) {
-    const G1Affine none = G1Affine::identity();
-    const uint32_t flags = s[0];
-    Fp x = fp_load_be(s, 0x1f);
-    if (!(flags & 0x80)) return {none, WHY_FLAGS};
-    if (flags & 0x40) return {none, (flags & 0x20) || !x.is_zero() ? WHY_FLAGS : WHY_IDENTITY};
-    if (!fp_is_canonical(x)) return {none, WHY_NONCANONICAL};
-    Fp xm = fp_from_canonical(x);
-    Root<Fp> y = fp_sqrt(xm.sqr() * xm + g1_b());
-    if (!y.ok) return {none, WHY_NOT_ON_CURVE};
-    if (fp_lexi_larger(y.v) != ((flags & 0x20) != 0)) y.v = y.v.neg();
-    G1Affine p{xm, y.v};
-    if (check_subgroup && !g1_in_subgroup(p)) return {none, WHY_NOT_IN_SUBGROUP};
-    return {p, WHY_OK};
-}
-
-BB_D Decoded<Fp2> g2_decode(const uint8_t* s, bool check_subgroup) {
-    const G2Affine none = G2Affine::identity();
-    const uint32_t flags = s[0];
-    Fp x1 = fp_load_be(s, 0x1f), x0 = fp_load_be(s + 48, 0xff);
-    if (!(flags & 0x80)) return {none, WHY_FLAGS};
-    if (flags & 0x40) return {none, (flags & 0x20) || !x0.is_zero() || !x1.is_zero() ? WHY_FLAGS : WHY_IDENTITY};
-    if (!fp_is_canonical(x0) || !fp_is_canonical(x1)) return {none, WHY_NONCANONICAL};
-    Fp2 xm{fp_from_canonical(x0), fp_from_canonical(x1)};
-    Root<Fp2> y = fp2_sqrt(xm.sqr() * xm + g2_b());
-    if (!y.ok) return {none, WHY_NOT_ON_CURVE};
-    if (fp2_lexi_larger(y.v) != ((flags & 0x20) != 0)) y.v = y.v.neg();
-    G2Affine p{xm, y.v};
-    if (check_subgroup && !g2_in_subgroup(p)) return {none, WHY_NOT_IN_SUBGROUP};
-    return {p, WHY_OK};
-}
 
 // point j of rows x parts: bytes base + (j % rows) * stride + (j / rows) * part_offset -> out[j / rows][j % rows]
 __global__ void __launch_bounds__(DECODE_THREADS) k_decode_g1(const uint8_t* __restrict__ base, size_t stride, size_t rows, size_t parts,
@@ -198,7 +43,7 @@ __global__ void __launch_bounds__(DECODE_THREADS) k_decode_g1(const uint8_t* __r
     size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= rows * parts) return;
     size_t row = j % rows, part = j / rows;
-    Decoded<Fp> d = g1_decode(base + row * stride + part * part_offset, check_subgroup != 0);
+    Decoded<Fp> d = decode_compressed<Fp>(base + row * stride + part * part_offset, check_subgroup != 0);
     (part ? out1 : out0)[row] = d.p;
     why[j] = (uint8_t)d.why;
 }
@@ -206,7 +51,7 @@ __global__ void __launch_bounds__(DECODE_THREADS) k_decode_g2(const uint8_t* __r
                                                               int check_subgroup, G2Affine* out, uint8_t* why) {
     size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= rows) return;
-    Decoded<Fp2> d = g2_decode(base + j * stride, check_subgroup != 0);
+    Decoded<Fp2> d = decode_compressed<Fp2>(base + j * stride, check_subgroup != 0);
     out[j] = d.p;
     why[j] = (uint8_t)d.why;
 }
@@ -226,68 +71,19 @@ __global__ void __launch_bounds__(128) k_proof_status(const uint8_t* __restrict_
 }
 
 // Proof::write (lib.rs:39-45): to_compressed of A, B, C
-BB_D void g1_encode(const G1Affine& p, uint8_t* o) {
-    if (p.is_identity()) { o[0] = 0xc0; for (int k = 1; k < 48; k++) o[k] = 0; return; }
-    fp_store_be(fp_to_canonical(p.x), o);
-    o[0] |= 0x80 | (fp_lexi_larger(p.y) ? 0x20 : 0);
-}
-BB_D void g2_encode(const G2Affine& p, uint8_t* o) {
-    if (p.is_identity()) { o[0] = 0xc0; for (int k = 1; k < 96; k++) o[k] = 0; return; }
-    fp_store_be(fp_to_canonical(p.x.c1), o);
-    fp_store_be(fp_to_canonical(p.x.c0), o + 48);
-    o[0] |= 0x80 | (fp2_lexi_larger(p.y) ? 0x20 : 0);
-}
 __global__ void __launch_bounds__(128) k_encode_proofs(const G1Affine* __restrict__ a, const G2Affine* __restrict__ b,
                                                        const G1Affine* __restrict__ c, size_t n, uint8_t* out) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     uint8_t* o = out + i * 192;
-    g1_encode(a[i], o);
-    g2_encode(b[i], o + 48);
-    g1_encode(c[i], o + 144);
+    encode_compressed(a[i], o);
+    encode_compressed(b[i], o + 48);
+    encode_compressed(c[i], o + 144);
 }
 
 constexpr size_t MAX_PROOFS = (size_t)1 << 31;
 
 // ---- Parameters::read: uncompressed points (from_uncompressed / _unchecked, then bellman's identity rule) ----------
-// why code of one point; *out = the Montgomery affine point (identity = zeros) when it is 0
-BB_D int g1_read_uncompressed(const uint8_t* s, bool checked, bool allow_identity, G1Affine* out) {
-    const uint32_t flags = s[0];
-    if (flags & 0xa0) return WHY_FLAGS;                                  // compression or sort bit
-    Fp x = fp_load_be(s, 0x1f), y = fp_load_be(s + 48, 0xff);
-    if (flags & 0x40) {
-        if (!x.is_zero() || !y.is_zero()) return WHY_FLAGS;
-        *out = G1Affine::identity();
-        return allow_identity ? WHY_OK : WHY_IDENTITY;
-    }
-    if (!fp_is_canonical(x) || !fp_is_canonical(y)) return WHY_NONCANONICAL;
-    G1Affine p{fp_from_canonical(x), fp_from_canonical(y)};
-    if (checked) {
-        if (p.y.sqr() != p.x.sqr() * p.x + g1_b()) return WHY_NOT_ON_CURVE;
-        if (!g1_in_subgroup(p)) return WHY_NOT_IN_SUBGROUP;
-    }
-    *out = p;
-    return WHY_OK;
-}
-BB_D int g2_read_uncompressed(const uint8_t* s, bool checked, bool allow_identity, G2Affine* out) {
-    const uint32_t flags = s[0];
-    if (flags & 0xa0) return WHY_FLAGS;
-    Fp x1 = fp_load_be(s, 0x1f), x0 = fp_load_be(s + 48, 0xff), y1 = fp_load_be(s + 96, 0xff), y0 = fp_load_be(s + 144, 0xff);
-    if (flags & 0x40) {
-        if (!x0.is_zero() || !x1.is_zero() || !y0.is_zero() || !y1.is_zero()) return WHY_FLAGS;
-        *out = G2Affine::identity();
-        return allow_identity ? WHY_OK : WHY_IDENTITY;
-    }
-    if (!fp_is_canonical(x0) || !fp_is_canonical(x1) || !fp_is_canonical(y0) || !fp_is_canonical(y1)) return WHY_NONCANONICAL;
-    G2Affine p{{fp_from_canonical(x0), fp_from_canonical(x1)}, {fp_from_canonical(y0), fp_from_canonical(y1)}};
-    if (checked) {
-        if (p.y.sqr() != p.x.sqr() * p.x + g2_b()) return WHY_NOT_ON_CURVE;
-        if (!g2_in_subgroup(p)) return WHY_NOT_IN_SUBGROUP;
-    }
-    *out = p;
-    return WHY_OK;
-}
-
 BB_D void first_failure(unsigned long long* first, unsigned long long code) {
 #if defined(__CUDACC__)
     atomicMin(first, code);
@@ -299,57 +95,44 @@ BB_D void first_failure(unsigned long long* first, unsigned long long code) {
 
 // n points at src (stride 96 / 192) -> out[0 .. n); point i has ordinal ord0 + i in the file.  A point behind the first
 // failure seen so far is skipped: only the first failure in file order is reported.
-__global__ void __launch_bounds__(DECODE_THREADS) k_params_decode_g1(const uint8_t* __restrict__ src, size_t n, uint64_t ord0, int checked,
-                                                                     int allow_identity, G1Affine* out, unsigned long long* first) {
+template <class F>
+BB_D void params_decode(const uint8_t* __restrict__ src, size_t n, uint64_t ord0, int checked, int allow_identity, Affine<F>* out,
+                        unsigned long long* first) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const unsigned long long ord = ord0 + i;
     if (*(volatile unsigned long long*)first < (ord << 3)) return;
-    G1Affine p;
-    int why = g1_read_uncompressed(src + i * 96, checked != 0, allow_identity != 0, &p);
+    Affine<F> p;
+    int why = read_uncompressed(src + i * 2 * sizeof(F), checked != 0, allow_identity != 0, &p);
     if (why) first_failure(first, (ord << 3) | (unsigned)why);
     else out[i] = p;
+}
+__global__ void __launch_bounds__(DECODE_THREADS) k_params_decode_g1(const uint8_t* __restrict__ src, size_t n, uint64_t ord0, int checked,
+                                                                     int allow_identity, G1Affine* out, unsigned long long* first) {
+    params_decode(src, n, ord0, checked, allow_identity, out, first);
 }
 __global__ void __launch_bounds__(DECODE_THREADS) k_params_decode_g2(const uint8_t* __restrict__ src, size_t n, uint64_t ord0, int checked,
                                                                      int allow_identity, G2Affine* out, unsigned long long* first) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const unsigned long long ord = ord0 + i;
-    if (*(volatile unsigned long long*)first < (ord << 3)) return;
-    G2Affine p;
-    int why = g2_read_uncompressed(src + i * 192, checked != 0, allow_identity != 0, &p);
-    if (why) first_failure(first, (ord << 3) | (unsigned)why);
-    else out[i] = p;
+    params_decode(src, n, ord0, checked, allow_identity, out, first);
 }
 
 // ---- Parameters::write (lib.rs:258-287): to_uncompressed, the inverse of the decoders above -----------------------------
-// canonical big-endian coordinates (G2: x.c1 | x.c0 | y.c1 | y.c0); the identity is the infinity flag 0x40, then zeros
-BB_D void g1_store_uncompressed(const G1Affine& p, uint8_t* o) {
-    if (p.is_identity()) { o[0] = 0x40; for (int k = 1; k < 96; k++) o[k] = 0; return; }
-    fp_store_be(fp_to_canonical(p.x), o);
-    fp_store_be(fp_to_canonical(p.y), o + 48);
-}
-BB_D void g2_store_uncompressed(const G2Affine& p, uint8_t* o) {
-    if (p.is_identity()) { o[0] = 0x40; for (int k = 1; k < 192; k++) o[k] = 0; return; }
-    fp_store_be(fp_to_canonical(p.x.c1), o);
-    fp_store_be(fp_to_canonical(p.x.c0), o + 48);
-    fp_store_be(fp_to_canonical(p.y.c1), o + 96);
-    fp_store_be(fp_to_canonical(p.y.c0), o + 144);
-}
 // n points -> out[0 .. 96 n) (G2: 192 n), one thread per point; prefix != 0: thread 0 also writes n as the big-endian u32 in
 // the four bytes before out (launched with at least one thread)
 BB_D void store_prefix(uint8_t* o, size_t n) {
     o[0] = (uint8_t)(n >> 24); o[1] = (uint8_t)(n >> 16); o[2] = (uint8_t)(n >> 8); o[3] = (uint8_t)n;
 }
-__global__ void __launch_bounds__(128) k_params_encode_g1(const G1Affine* __restrict__ pts, size_t n, int prefix, uint8_t* out) {
+template <class F>
+BB_D void params_encode(const Affine<F>* __restrict__ pts, size_t n, int prefix, uint8_t* out) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (prefix && i == 0) store_prefix(out - 4, n);
-    if (i < n) g1_store_uncompressed(pts[i], out + i * 96);
+    if (i < n) store_uncompressed(pts[i], out + i * 2 * sizeof(F));
+}
+__global__ void __launch_bounds__(128) k_params_encode_g1(const G1Affine* __restrict__ pts, size_t n, int prefix, uint8_t* out) {
+    params_encode(pts, n, prefix, out);
 }
 __global__ void __launch_bounds__(128) k_params_encode_g2(const G2Affine* __restrict__ pts, size_t n, int prefix, uint8_t* out) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (prefix && i == 0) store_prefix(out - 4, n);
-    if (i < n) g2_store_uncompressed(pts[i], out + i * 192);
+    params_encode(pts, n, prefix, out);
 }
 
 constexpr int PARAMS_SECTIONS = 12, VK_SECTIONS = 7;

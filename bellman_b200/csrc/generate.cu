@@ -21,6 +21,7 @@
 #include <deque>
 
 #include "bb_internal.cuh"
+#include "encoding.cuh"
 
 using namespace bb;
 
@@ -182,26 +183,13 @@ bool fr_below_r(const Fr& v) {
     return false;
 }
 
-template <class F> bool coords_canonical(const F& v);
-template <> bool coords_canonical(const Fp& v) {
-    for (int i = 11; i >= 0; i--) {
-        if (v.l[i] != bbc::FP_MOD[i]) return v.l[i] < bbc::FP_MOD[i];
-    }
-    return false;
-}
-template <> bool coords_canonical(const Fp2& v) { return coords_canonical(v.c0) && coords_canonical(v.c1); }
-
-Fp curve_b(const Fp*) { Fp four = Fp::zero(); four.l[0] = 4; return fp_from_canonical(four); }
-Fp2 curve_b(const Fp2*) { const Fp b = curve_b((const Fp*)nullptr); return {b, b}; }
-
 // the checks the reference's types guarantee for a generator: a non-identity point of order r on the curve
 template <class F>
 const char* bad_generator(const Affine<F>& p) {
-    if (!coords_canonical(p.x) || !coords_canonical(p.y)) return "a coordinate is not below p";
+    if (!is_canonical(p.x) || !is_canonical(p.y)) return "a coordinate is not below p";
     if (p.is_identity()) return "the identity";
-    if (p.y.sqr() != p.x.sqr() * p.x + curve_b((const F*)nullptr)) return "not on the curve";
-    const uint32_t r[8] = {BBC_FR_MOD_LIST};
-    if (!XYZZ<F>::from_affine(p).mul_bits(r).is_identity()) return "not in the prime-order subgroup";
+    if (!on_curve(p)) return "not on the curve";
+    if (!rP_is_identity(p)) return "not in the prime-order subgroup";
     return nullptr;
 }
 

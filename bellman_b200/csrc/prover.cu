@@ -12,6 +12,7 @@
 #include <thread>
 
 #include "bb_internal.cuh"
+#include "encoding.cuh"
 
 using namespace bb;
 
@@ -90,38 +91,9 @@ XYZZ<F> host_mul(const XYZZ<F>& p, const uint32_t* k_in) {
     return acc;
 }
 
-void fp_to_be(const Fp& v, uint8_t* out) {
-    Fp c = fp_to_canonical(v);
-    for (int i = 0; i < 12; i++)
-        for (int b = 0; b < 4; b++) out[47 - (4 * i + b)] = (uint8_t)(c.l[i] >> (8 * b));
-}
-bool fp_lexi_larger(const Fp& v) {               // canonical(v) > (p-1)/2
-    static const uint32_t half[12] = {BBC_FP_HALF_LIST};
-    Fp c = fp_to_canonical(v);
-    for (int i = 11; i >= 0; i--) {
-        if (c.l[i] > half[i]) return true;
-        if (c.l[i] < half[i]) return false;
-    }
-    return false;
-}
-
 }  // namespace
 
 namespace bb {
-void g1_compress(const G1Affine& p, uint8_t* out) {
-    if (p.is_identity()) { std::memset(out, 0, 48); out[0] = 0xC0; return; }
-    fp_to_be(p.x, out);
-    out[0] |= 0x80;
-    if (fp_lexi_larger(p.y)) out[0] |= 0x20;
-}
-void g2_compress(const G2Affine& p, uint8_t* out) {
-    if (p.is_identity()) { std::memset(out, 0, 96); out[0] = 0xC0; return; }
-    fp_to_be(p.x.c1, out);
-    fp_to_be(p.x.c0, out + 48);
-    out[0] |= 0x80;
-    bool larger = p.y.c1.is_zero() ? fp_lexi_larger(p.y.c0) : fp_lexi_larger(p.y.c1);
-    if (larger) out[0] |= 0x20;
-}
 G1X g1_host_mul(const G1X& p, const uint32_t* k) { return host_mul<Fp>(p, k); }
 G2X g2_host_mul(const G2X& p, const uint32_t* k) { return host_mul<Fp2>(p, k); }
 }  // namespace bb
@@ -564,9 +536,9 @@ int finalize_impl(const bb_crs* crs, const uint8_t* partials, size_t count, cons
     G1X ac[2] = {g_a, g_c};                                                       // :356-360: to_affine, one inversion for A and C
     G1Affine ac_aff[2];
     batch_to_affine<Fp>(ac, 2, ac_aff);
-    g1_compress(ac_aff[0], proof);                                                // lib.rs:39-45
-    g2_compress(g_b.to_affine(), proof + 48);
-    g1_compress(ac_aff[1], proof + 144);
+    encode_compressed(ac_aff[0], proof);                                          // lib.rs:39-45
+    encode_compressed(g_b.to_affine(), proof + 48);
+    encode_compressed(ac_aff[1], proof + 144);
     return BB_OK;
 }
 

@@ -260,6 +260,15 @@ def test_errors(worker):
             GEN.generate_parameters_device(worker, r1cs, *tox, g1=bad_g1)
     with pytest.raises(bb.BackendError, match="identity"):
         GEN.generate_parameters_device(worker, r1cs, *tox, g2=np.zeros(24, np.uint64))
+    p_limbs = np.array([(F.FP_MODULUS >> (64 * k)) % (1 << 64) for k in range(6)], np.uint64)
+    x_is_p = g1.copy()
+    x_is_p[:6] = p_limbs
+    with pytest.raises(bb.BackendError, match="not below p"):
+        GEN.generate_parameters_device(worker, r1cs, *tox, g1=x_is_p)
+    y1_is_p = o1.g2_fixed_mul(o1.fr_from_ints([3]))[0].copy()
+    y1_is_p[18:] = p_limbs                                     # y.c1, the last of x.c0 | x.c1 | y.c0 | y.c1
+    with pytest.raises(bb.BackendError, match="not below p"):
+        GEN.generate_parameters_device(worker, r1cs, *tox, g2=y1_is_p)
     from test_gpu_proof_read import off_subgroup_g1, off_subgroup_g2
     with pytest.raises(bb.BackendError, match="subgroup"):
         GEN.generate_parameters_device(worker, r1cs, *tox, g1=o1.g1_from_affine_ints([off_subgroup_g1(rng)])[0])

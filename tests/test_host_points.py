@@ -48,3 +48,16 @@ def test_point_add_mul_compress_host():
         for i in range(len(ks)):
             assert bb.point_compress(group, pts[i:i + 1]) == bytes(want[i])
         assert bb.point_compress(group, zero) == bytes([0xC0] + [0] * (47 if group == bb.G1 else 95))
+
+
+def test_compress_g2_real_y_host():
+    """G2 points with y.c1 = 0: the sort bit comes from y.c0, both signs"""
+    from oracle.oracle0 import fields as F
+    from test_gpu_proof_read import g2_points_with_real_y
+    pts = g2_points_with_real_y(random.Random(11), 3)
+    pts += [F.G2.neg(p) for p in pts]
+    abi = o1.g2_from_affine_ints(pts)
+    want = o1.g2_compress(abi)
+    assert len({bytes(w)[0] & 0x20 for w in want}) == 2                                               # both signs present
+    for i in range(len(pts)):
+        assert bb.point_compress(bb.G2, abi[i:i + 1]) == bytes(want[i])
