@@ -157,23 +157,27 @@ int device_input(bb_ctx* ctx, cudaStream_t st, const void* p, size_t bytes, bool
 
 // CUDA-event brackets of a call's stages (profile mode only)
 struct StageTimer {
+    static constexpr uint64_t REPORT_UNITS = ~0ull;          // a mark without units of its own: report()'s
     bb_ctx* ctx;
     cudaStream_t st;
     std::vector<std::pair<const char*, cudaEvent_t>> marks;
+    std::vector<uint64_t> mark_units;
     StageTimer(bb_ctx* c, cudaStream_t s) : ctx(c), st(s) {}
     ~StageTimer() { for (auto& m : marks) cudaEventDestroy(m.second); }
-    void mark(const char* stage_ending_here) {
+    void mark(const char* stage_ending_here, uint64_t units = REPORT_UNITS) {
         if (!ctx->opt_profile) return;
         cudaEvent_t e;
         if (cudaEventCreate(&e) != cudaSuccess) return;
         cudaEventRecord(e, st);
         marks.emplace_back(stage_ending_here, e);
+        mark_units.push_back(units);
     }
     // after the stream has drained: stage k = the interval between marks k-1 and k
     void report(uint64_t units) {
         for (size_t k = 1; k < marks.size(); k++) {
             float ms = 0;
-            if (cudaEventElapsedTime(&ms, marks[k - 1].second, marks[k].second) == cudaSuccess) ctx->prof_add(marks[k].first, ms, 1, units);
+            if (cudaEventElapsedTime(&ms, marks[k - 1].second, marks[k].second) == cudaSuccess)
+                ctx->prof_add(marks[k].first, ms, 1, mark_units[k] == REPORT_UNITS ? units : mark_units[k]);
         }
     }
 };
@@ -203,6 +207,25 @@ int prove_batch_impl(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t
                      uint8_t* proofs, int* status, const BatchAbcFill* fill = nullptr);
 int prove_batch_check(const char* fn, const bb_ctx* ctx, const bb_crs* crs, size_t count, const void* r, const void* s, const void* proofs,
                       const int* status);
+// Queues on the main stream, after the witness upload and ahead of the witness MSMs, the owner stage of a proof from a
+// resident constraint system: d_in / d_aux the witness on the device, tmp m Fr of scratch, tm its profile-mode stages
+using ProveHead = std::function<int(cudaStream_t st, const Fr* d_in, const Fr* d_aux, Fr* tmp, StageTimer& tm)>;
+// How bb_groth16_prove_r1cs_begin starts a proof (its witness, device or host, is read in place or uploaded once).  split:
+// `head` (empty: nothing is owned) runs ahead of the witness MSMs and bb_groth16_prove_end takes the three vectors.
+// Otherwise `fill` (B = 1) evaluates a, b, c into the H pipeline's rows, and the H pipeline and the h MSM are queued ahead
+// of the witness MSMs; bb_groth16_prove_end takes no vectors.  units: the terms of the three matrices, the profile-mode
+// units of the replicated mode's r1cs.upload and r1cs.eval stages.
+struct R1csStart {
+    bool split;
+    ProveHead head;
+    BatchAbcFill fill;
+    uint64_t units;
+};
+int prove_begin_r1cs(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, const R1csStart& start, bb_prove** out);
+// bb_groth16_prove after its argument checks: `begin` queues the proof on an unsharded key, the scalar multiplications
+// that need no MSM result run on the host meanwhile, then the waits and the finalisation
+int prove_single(bb_ctx* ctx, const bb_crs* crs, const std::function<int(bb_prove**)>& begin, const uint8_t* r, const uint8_t* s,
+                 uint8_t* proof);
 // A single-GPU bb_crs that adopts the five resident vectors h, l, a, b_g1, b_g2 (freed with it); g1 = alpha, beta, delta,
 // g2 = beta, delta (bb_params_read)
 bb_crs* crs_adopt(bb_ctx* ctx, bb_bases* const vec[5], const G1Affine g1[3], const G2Affine g2[2]);

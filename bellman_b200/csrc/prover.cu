@@ -300,6 +300,11 @@ struct bb_prove {
     size_t m;
     uint32_t log_m;
     DevBuf d_abc, d_tmp, d_in, d_aux;             // d_abc: rows a_0 .. a_{B-1}, b_0 .., c_0 .. of m Fr; item i's h ends in a_i
+    bool in_place = false;                        // B = 1, device witness: the MSMs and the evaluation read the caller's arrays
+    const Fr *in_p = nullptr, *aux_p = nullptr;   // the witnesses on the device: d_in / d_aux, or the caller's arrays
+    int end_evals = 0;                            // bb_groth16_prove_end: 0 = with the three vectors or without, 1 = with, -1 = without
+    std::unique_ptr<StageTimer> tm;               // profile mode: the r1cs.* or r1cs_owner.* stages of a proof from the witness
+    uint64_t r1cs_terms = 0;                      // the units of the r1cs.* stages
     cudaStream_t up = nullptr;
     cudaEvent_t ev_up = nullptr, ev_h = nullptr;
     Slot slot[8];
@@ -348,13 +353,19 @@ int h_pipeline(bb_prove* P, const void* const* evals, const BatchAbcFill* fill) 
     cudaStream_t st = ctx->main_stream;
     const bb_witness& w0 = P->w[0];
     const size_t n = w0.n_constraints, m = P->m, B = P->B;
-    BB_TRY(P->d_tmp.alloc(ctx, (P->batched ? 3 * B : 1) * m * 32));
+    if (!P->d_tmp.p) BB_TRY(P->d_tmp.alloc(ctx, (P->batched ? 3 * B : 1) * m * 32));     // (an owner stage may have made it)
     if (evals) return h_poly_final_device(ctx, st, (Fr*)evals[0], (const Fr*)evals[1], (const Fr*)evals[2], P->d_tmp.as<Fr>(), P->log_m);
     BB_TRY(P->d_abc.alloc(ctx, 3 * B * m * 32));
     Fr* abc = P->d_abc.as<Fr>();
     if (fill) {                                          // a, b, c evaluated on the device from the uploaded witnesses
+        if (!P->batched) {                               // bb_groth16_prove_r1cs's stages (bb_profile_read)
+            P->tm.reset(new StageTimer(ctx, st));
+            P->tm->mark("r1cs.begin");
+        }
         BB_CUDA(cudaStreamWaitEvent(st, P->ev_up, 0));
-        BB_TRY((*fill)(st, (uint32_t)B, abc, m, P->d_in.as<Fr>(), P->d_aux.as<Fr>()));
+        if (P->tm) P->tm->mark("r1cs.upload", P->r1cs_terms);
+        BB_TRY((*fill)(st, (uint32_t)B, abc, m, P->in_p, P->aux_p));
+        if (P->tm) P->tm->mark("r1cs.eval", P->r1cs_terms);
     } else {
         for (size_t i = 0; i < B; i++) {
             const void* srcs[3] = {P->w[i].a, P->w[i].b, P->w[i].c};
@@ -383,23 +394,41 @@ int prove_queue_h(bb_prove* P, const void* const* evals, const BatchAbcFill* fil
 // Queues the uploads and the MSMs of the B proofs (prover.rs:221-318).  h_inline: the H pipeline and the h MSM are queued
 // here, FIRST -- they are the longest dependency chain of a proof and run on high-priority streams, the seven witness MSMs
 // fill the machine around them.  Otherwise prove_end queues them (multi-GPU: the coset evaluations arrive from other ranks
-// while the witness MSMs already run).  A failure to queue a job is kept in P->s.
-int prove_queue(bb_prove* P, bool h_inline, const BatchAbcFill* fill) {
+// while the witness MSMs already run); `head`, if any, is queued on the main stream behind the upload and ahead of the
+// witness MSMs (the owner stage of bb_groth16_prove_r1cs_begin; a failure to queue it fails the call).  A failure to queue a
+// job is kept in P->s.
+int prove_queue(bb_prove* P, bool h_inline, const BatchAbcFill* fill, const ProveHead* head = nullptr) {
     bb_ctx* ctx = P->ctx;
     const bb_witness& w0 = P->w[0];
     const size_t ni = w0.n_inputs, na = w0.n_aux, B = P->B;
-    BB_TRY(P->d_in.alloc(ctx, B * ni * 32)); BB_TRY(P->d_aux.alloc(ctx, B * na * 32));
     P->up = ctx->pick_stream();
     BB_CUDA(cudaEventCreateWithFlags(&P->ev_up, cudaEventDisableTiming));
     BB_CUDA(cudaEventCreateWithFlags(&P->ev_h, cudaEventDisableTiming));
-    const cudaMemcpyKind kind = w0.on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    for (size_t i = 0; i < B; i++) {
-        if (ni) BB_CUDA(cudaMemcpyAsync((char*)P->d_in.p + i * ni * 32, P->w[i].input_assignment, ni * 32, kind, P->up));
-        if (na) BB_CUDA(cudaMemcpyAsync((char*)P->d_aux.p + i * na * 32, P->w[i].aux_assignment, na * 32, kind, P->up));
+    if (P->in_place) {
+        P->in_p = (const Fr*)w0.input_assignment;
+        P->aux_p = (const Fr*)(na ? w0.aux_assignment : w0.input_assignment);      // no aux: never read
+    } else {
+        BB_TRY(P->d_in.alloc(ctx, B * ni * 32)); BB_TRY(P->d_aux.alloc(ctx, B * na * 32));
+        const cudaMemcpyKind kind = w0.on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+        for (size_t i = 0; i < B; i++) {
+            if (ni) BB_CUDA(cudaMemcpyAsync((char*)P->d_in.p + i * ni * 32, P->w[i].input_assignment, ni * 32, kind, P->up));
+            if (na) BB_CUDA(cudaMemcpyAsync((char*)P->d_aux.p + i * na * 32, P->w[i].aux_assignment, na * 32, kind, P->up));
+        }
+        if (!w0.on_device) ctx->h2d_bytes += B * (ni + na) * 32;
+        P->in_p = P->d_in.as<Fr>();
+        P->aux_p = P->d_aux.as<Fr>();
     }
-    if (!w0.on_device) ctx->h2d_bytes += B * (ni + na) * 32;
     BB_CUDA(cudaEventRecord(P->ev_up, P->up));
-    slot_table(P->crs, w0, P->m, P->d_in.p, P->d_aux.p, P->slot);
+    slot_table(P->crs, w0, P->m, P->in_p, P->aux_p, P->slot);
+    if (head) {
+        cudaStream_t st = ctx->main_stream;
+        P->tm.reset(new StageTimer(ctx, st));
+        P->tm->mark("r1cs_owner.begin");
+        BB_CUDA(cudaStreamWaitEvent(st, P->ev_up, 0));
+        P->tm->mark("r1cs_owner.upload", 0);
+        BB_TRY(P->d_tmp.alloc(ctx, P->m * 32));
+        BB_TRY((*head)(st, P->in_p, P->aux_p, P->d_tmp.as<Fr>(), *P->tm));
+    }
     if (h_inline) prove_queue_h(P, nullptr, fill);
     // all eight MSMs are in flight before the first wait (prover.rs:244-318); the G2 MSM has the longest chain of the seven
     // (Fp2 arithmetic): it goes first, on the other high-priority stream
@@ -450,7 +479,8 @@ void write_partials(const bb_prove* P, const std::vector<uint32_t>& items, uint8
     }
 }
 
-int prove_begin_impl(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, bool h_inline, bb_prove** out) {
+// r1cs: a proof from a resident constraint system (bb_groth16_prove_r1cs_begin), NULL for bb_groth16_prove_begin's
+int prove_begin_impl(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, bool h_inline, bb_prove** out, const R1csStart* r1cs = nullptr) {
     NvtxRange range("bb: prove_begin (uploads, queue MSMs)");
     if (!ctx || !crs || !w || !out) { set_error("bb_groth16_prove: null argument"); return BB_ERR_ARG; }
     BB_CUDA(cudaSetDevice(ctx->device));
@@ -459,7 +489,14 @@ int prove_begin_impl(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, bool h
     BB_TRY(domain_size(w->n_constraints, &m, &log_m));
     BB_TRY(profile_epoch(ctx));
     std::unique_ptr<bb_prove> P(new bb_prove(ctx, crs, w, 1, false, m, log_m));
-    BB_TRY(prove_queue(P.get(), h_inline, nullptr));
+    if (r1cs) {
+        P->in_place = w->on_device != 0;
+        P->end_evals = r1cs->split ? 1 : -1;
+        P->r1cs_terms = r1cs->units;
+        BB_TRY(prove_queue(P.get(), !r1cs->split, r1cs->split ? nullptr : &r1cs->fill, r1cs->head ? &r1cs->head : nullptr));
+    } else {
+        BB_TRY(prove_queue(P.get(), h_inline, nullptr));
+    }
     *out = P.release();
     return BB_OK;
 }
@@ -470,10 +507,16 @@ int prove_end_impl(bb_prove* Praw, const void* const* evals, uint8_t* partials) 
     NvtxRange range("bb: prove_end (waits, folds)");
     std::unique_ptr<bb_prove> P(Praw);
     if (!Praw || !partials) { set_error("bb_groth16_prove_end: null argument"); return BB_ERR_ARG; }
+    if ((P->end_evals > 0 && !evals) || (P->end_evals < 0 && evals)) {
+        set_error("bb_groth16_prove_end: %s", evals ? "this proof ran its whole H pipeline in bb_groth16_prove_r1cs_begin: no evaluation vectors"
+                                                    : "this proof's H pipeline was split by polynomial: the three evaluation vectors are needed");
+        return BB_ERR_ARG;
+    }
     BB_CUDA(cudaSetDevice(P->ctx->device));
     if (!P->h_queued && P->s == BB_OK) prove_queue_h(P.get(), evals, nullptr);
     int job_status[8];
     prove_wait(P.get(), job_status);
+    if (P->tm && P->ctx->opt_profile && cudaStreamSynchronize(P->ctx->main_stream) == cudaSuccess) P->tm->report(0);
     if (P->s != BB_OK) return P->s;
     const int s = proof_status(P->status.data(), 1, delta_is_identity(P->crs));
     if (s != BB_OK) return prove_error(P->crs, s);
@@ -750,8 +793,15 @@ int bb_h_coset_evals_wait(bb_ctx* ctx) {
 }
 
 int bb_h_coset_evals(bb_ctx* ctx, const void* poly, size_t n_constraints, int on_device, void* d_out) {
+    std::unique_ptr<StageTimer> tm;                       // profile mode: the stage h_coset_evals (copy, padding, transforms)
+    if (ctx && ctx->opt_profile && cudaSetDevice(ctx->device) == cudaSuccess) {
+        tm.reset(new StageTimer(ctx, ctx->main_stream));
+        tm->mark("h_coset_evals.begin");
+    }
     int s = bb_h_coset_evals_async(ctx, poly, n_constraints, on_device, d_out);
+    if (tm) tm->mark("h_coset_evals");
     int w = ctx ? bb_h_coset_evals_wait(ctx) : BB_OK;
+    if (tm && s == BB_OK && w == BB_OK) tm->report(n_constraints);
     return s != BB_OK ? s : w;
 }
 
@@ -896,6 +946,28 @@ int bb_groth16_autotune(bb_ctx* ctx, bb_crs* crs, const bb_witness* w, int reps,
 int bb_groth16_prove(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, const uint8_t* r_bytes, const uint8_t* s_bytes, uint8_t* proof) {
     if (!crs || !r_bytes || !s_bytes || !proof) { set_error("bb_groth16_prove: null argument"); return BB_ERR_ARG; }
     if (crs->shard_count != 1) { set_error("bb_groth16_prove needs an unsharded CRS; use prove_partials + finalize"); return BB_ERR_ARG; }
+    return prove_single(ctx, crs, [&](bb_prove** P) { return prove_begin_impl(ctx, crs, w, true, P); }, r_bytes, s_bytes, proof);
+}
+
+const char* bb_groth16_prove_message(const bb_crs* crs, int status) { return crs ? prove_status_message(crs, status) : nullptr; }
+
+int bb_groth16_prove_batch(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t count, const uint8_t* r, const uint8_t* s,
+                           uint8_t* proofs, int* status) {
+    return prove_batch_impl(ctx, crs, w, count, r, s, proofs, status);
+}
+
+}  // extern "C"
+
+namespace bb {
+
+int prove_begin_r1cs(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, const R1csStart& start, bb_prove** out) {
+    return prove_begin_impl(ctx, crs, w, false, out, &start);
+}
+
+// one proof on an unsharded key: `begin` queues it, the five scalar multiplications that need no MSM result run on the
+// host meanwhile, then the waits and the finalisation
+int prove_single(bb_ctx* ctx, const bb_crs* crs, const std::function<int(bb_prove**)>& begin, const uint8_t* r_bytes, const uint8_t* s_bytes,
+                 uint8_t* proof) {
     uint8_t partials[BB_PARTIALS_BYTES];
     std::memset(partials, 0, sizeof partials);
     Fr r, s;
@@ -905,7 +977,7 @@ int bb_groth16_prove(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, const 
     const auto t_entry = std::chrono::steady_clock::now();
     auto since = [&] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_entry).count(); };
     bb_prove* P = nullptr;
-    BB_TRY(prove_begin_impl(ctx, crs, w, true, &P));
+    BB_TRY(begin(&P));
     const double t_queued = since();
     // the five scalar multiplications that need no MSM result run on the host while the device works
     ProofStatic stat;
@@ -923,11 +995,4 @@ int bb_groth16_prove(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, const 
     return rc;
 }
 
-const char* bb_groth16_prove_message(const bb_crs* crs, int status) { return crs ? prove_status_message(crs, status) : nullptr; }
-
-int bb_groth16_prove_batch(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, size_t count, const uint8_t* r, const uint8_t* s,
-                           uint8_t* proofs, int* status) {
-    return prove_batch_impl(ctx, crs, w, count, r, s, proofs, status);
-}
-
-}  // extern "C"
+}  // namespace bb

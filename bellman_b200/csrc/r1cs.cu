@@ -13,7 +13,9 @@
 //   position; terms with coefficient zero are dropped (they add nothing, and the densities are
 //   taken before);
 //   the row ids binned by length: <= 32 terms one thread per row, 33..2048 one warp per row,
-//   more one CTA of 256 threads per row.
+//   more one CTA of 256 threads per row.  Each bin lists its rows in ascending g, so the rows of
+//   one matrix are one contiguous run inside each bin: bin_rows[bin][matrix] counts them, and the
+//   owner of one polynomial evaluates its matrix alone over those runs (bb_groth16_prove_r1cs_begin).
 #include <algorithm>
 #include <memory>
 #include <vector>
@@ -81,6 +83,18 @@ __global__ void __launch_bounds__(GROUP_THREADS) k_r1cs_rows_group(EvalArgs A, c
     if (lane == 0 && slot < count) r1cs_put(A, g, sh[threadIdx.x]);
 }
 
+// The three row kernels on `st`: count[b] rows listed at rows[b] for the short, warp and CTA bin; an empty bin is not launched
+int rows_queue(bb_ctx* ctx, cudaStream_t st, const EvalArgs& A, const uint32_t* const rows[3], const uint32_t count[3]) {
+    if (count[0]) { k_r1cs_rows_thread<<<cdiv(count[0], 128), 128, 0, st>>>(A, rows[0], count[0]); ctx->count_launch(); }
+    if (count[1]) {
+        k_r1cs_rows_group<32><<<cdiv(count[1], GROUP_THREADS / 32), GROUP_THREADS, 0, st>>>(A, rows[1], count[1]);
+        ctx->count_launch();
+    }
+    if (count[2]) { k_r1cs_rows_group<GROUP_THREADS><<<count[2], GROUP_THREADS, 0, st>>>(A, rows[2], count[2]); ctx->count_launch(); }
+    BB_CUDA(cudaGetLastError());
+    return BB_OK;
+}
+
 // which_is_unsatisfied over evaluated rows: row k fails when a[k] b[k] != c[k] (Montgomery product, limb equality; every
 // value is below r).  A failing row lowers *first, counts itself in *count and, with bits, sets bit k of the LSB-first
 // words (the uint64 density words' bytes).  A satisfied witness issues no atomics.
@@ -111,6 +125,7 @@ struct bb_r1cs {
     std::vector<uint64_t> a_aux_density, b_input_density, b_aux_density;
     void *d_off = nullptr, *d_idx = nullptr, *d_coef = nullptr, *d_rows = nullptr;
     uint32_t n_short = 0, n_warp = 0, n_cta = 0;
+    uint32_t bin_rows[3][3] = {};                        // [bin][matrix]: rows of matrix A, B, C in the short, warp, CTA bin
     ~bb_r1cs() {
         for (void* p : {d_off, d_idx, d_coef, d_rows})
             if (p) ctx->release(p);
@@ -149,6 +164,54 @@ int r1cs_eval_queue(bb_ctx* ctx, cudaStream_t st, const bb_r1cs* R, const Fr* d_
     const CsrMatrix M{(const uint32_t*)R->d_off, (const uint32_t*)R->d_idx, (const Fr*)R->d_coef, (const uint32_t*)R->d_rows,
                       R->n_short, R->n_warp, R->n_cta, (uint32_t)R->n};
     return csr_eval_queue(ctx, st, M, d_in, (uint32_t)R->n_inputs, d_aux, oa, ob, oc);
+}
+
+// The owner stage of polynomial i (0 = a, 1 = b, 2 = c) on `st`: <M_i,k, z> for k < n straight into out (m Fr) over matrix
+// i's runs of the three bins -- the other two matrices are not read -- zeros up to m (domain.rs:69), then ifft + coset_fft
+// in place (prover.rs:225-230) with tmp (m Fr) as scratch
+int r1cs_owner_queue(bb_ctx* ctx, cudaStream_t st, const bb_r1cs* R, int i, const Fr* d_in, const Fr* d_aux, Fr* out, size_t m, uint32_t log_m,
+                     Fr* tmp, StageTimer& tm) {
+    const size_t n = R->n;
+    const EvalArgs A{(const uint32_t*)R->d_off, (const uint32_t*)R->d_idx, (const Fr*)R->d_coef, d_in, d_aux, out, out, out,
+                     (uint32_t)R->n_inputs, (uint32_t)n};     // matrix i's rows land in out whichever output r1cs_put picks
+    const uint32_t* order = (const uint32_t*)R->d_rows;
+    const uint32_t bin_start[3] = {0, R->n_short, R->n_short + R->n_warp};
+    const uint32_t* rows[3];
+    uint32_t count[3];
+    for (int b = 0; b < 3; b++) {
+        uint32_t lo = bin_start[b];
+        for (int q = 0; q < i; q++) lo += R->bin_rows[b][q];
+        rows[b] = order + lo;
+        count[b] = R->bin_rows[b][i];
+    }
+    BB_TRY(rows_queue(ctx, st, A, rows, count));
+    if (m > n) BB_CUDA(cudaMemsetAsync(out + n, 0, (m - n) * 32, st));
+    tm.mark("r1cs_owner.eval", R->nnz[i]);
+    BB_TRY(h_poly_evals_device(ctx, st, out, tmp, log_m));
+    tm.mark("r1cs_owner.transforms", m);
+    return BB_OK;
+}
+
+// The bb_witness bb_groth16_prove would take for this witness, without a, b, c
+bb_witness r1cs_witness(const bb_r1cs* R, const void* input, const void* aux, int on_device) {
+    bb_witness w{};
+    w.n_constraints = R->n;
+    w.input_assignment = input; w.n_inputs = R->n_inputs;
+    w.aux_assignment = aux; w.n_aux = R->n_aux;
+    w.a_aux_density = R->a_aux_density.data();
+    w.b_input_density = R->b_input_density.data();
+    w.b_aux_density = R->b_aux_density.data();
+    w.on_device = on_device;
+    return w;
+}
+
+// The replicated start: a, b, c into the H pipeline's rows (stride m) by the combined bins
+R1csStart r1cs_replicated(bb_ctx* ctx, const bb_r1cs* R) {
+    R1csStart st{false, {}, {}, R->nnz[0] + R->nnz[1] + R->nnz[2]};
+    st.fill = [ctx, R](cudaStream_t s, uint32_t, Fr* abc, size_t m, const Fr* d_in, const Fr* d_aux) -> int {
+        return r1cs_eval_queue(ctx, s, R, d_in, d_aux, abc, abc + m, abc + 2 * m);
+    };
+    return st;
 }
 
 // bb_r1cs_check(_batch) after the argument checks: `count` witnesses (row-major, bb_groth16_prove_r1cs_batch's layout)
@@ -215,19 +278,10 @@ namespace bb {
 
 int csr_eval_queue(bb_ctx* ctx, cudaStream_t st, const CsrMatrix& M, const Fr* input, uint32_t n_inputs, const Fr* aux, Fr* oa, Fr* ob,
                    Fr* oc) {
-    EvalArgs A{M.off, M.idx, M.coef, input, aux, oa, ob, oc, n_inputs, M.n};
-    const uint32_t* rows = M.rows;
-    if (M.n_short) { k_r1cs_rows_thread<<<cdiv(M.n_short, 128), 128, 0, st>>>(A, rows, M.n_short); ctx->count_launch(); }
-    if (M.n_warp) {
-        k_r1cs_rows_group<32><<<cdiv(M.n_warp, GROUP_THREADS / 32), GROUP_THREADS, 0, st>>>(A, rows + M.n_short, M.n_warp);
-        ctx->count_launch();
-    }
-    if (M.n_cta) {
-        k_r1cs_rows_group<GROUP_THREADS><<<M.n_cta, GROUP_THREADS, 0, st>>>(A, rows + M.n_short + M.n_warp, M.n_cta);
-        ctx->count_launch();
-    }
-    BB_CUDA(cudaGetLastError());
-    return BB_OK;
+    const EvalArgs A{M.off, M.idx, M.coef, input, aux, oa, ob, oc, n_inputs, M.n};
+    const uint32_t* const rows[3] = {M.rows, M.rows + M.n_short, M.rows + M.n_short + M.n_warp};
+    const uint32_t count[3] = {M.n_short, M.n_warp, M.n_cta};
+    return rows_queue(ctx, st, A, rows, count);
 }
 
 R1csView r1cs_view(const bb_r1cs* R) {
@@ -304,6 +358,11 @@ int bb_r1cs_create(bb_ctx* ctx, const bb_r1cs_desc* d, bb_r1cs** out) {
             bin(g, idx.size() - off[g]);
         }
         R->nnz[m] = idx.size() - off[(size_t)m * n];
+        for (int b = 0; b < 3; b++) {                            // this matrix's run in each bin: what the bin gained since the last matrix
+            uint32_t before = 0;
+            for (int q = 0; q < m; q++) before += R->bin_rows[b][q];
+            R->bin_rows[b][m] = (uint32_t)rbins[b].size() - before;
+        }
     }
     off[3 * n] = (uint32_t)idx.size();
     R->n_short = (uint32_t)rbins[0].size(); R->n_warp = (uint32_t)rbins[1].size(); R->n_cta = (uint32_t)rbins[2].size();
@@ -380,35 +439,44 @@ int bb_groth16_prove_r1cs(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* R, cons
                           size_t n_aux, int on_device, const uint8_t r[32], const uint8_t s[32], uint8_t proof[192]) {
     if (!ctx || !crs || !R || !r || !s || !proof) { set_error("bb_groth16_prove_r1cs: null argument"); return BB_ERR_ARG; }
     BB_TRY(check_witness("bb_groth16_prove_r1cs", ctx, R, input, n_inputs, aux, n_aux, on_device, true));
+    if (crs_view(crs).shard_count != 1) { set_error("bb_groth16_prove needs an unsharded CRS; use prove_partials + finalize"); return BB_ERR_ARG; }
+    NvtxRange nvtx("prove_r1cs");
+    // create_proof from here on (prover.rs:217-360): the H pipeline evaluates a, b, c on its own stream after the upload,
+    // the witness MSMs do not wait for the evaluation
+    const bb_witness w = r1cs_witness(R, input, aux, on_device);
+    const R1csStart start = r1cs_replicated(ctx, R);
+    return prove_single(ctx, crs, [&](bb_prove** P) { return prove_begin_r1cs(ctx, crs, &w, start, P); }, r, s, proof);
+}
+
+int bb_groth16_prove_r1cs_begin(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* R, const void* input, size_t n_inputs, const void* aux,
+                                size_t n_aux, int on_device, unsigned own, void* const d_evals[3], bb_prove** out) {
+    static const char* const fn = "bb_groth16_prove_r1cs_begin";
+    if (out) *out = nullptr;
+    if (!ctx || !crs || !R || !out) { set_error("%s: null argument", fn); return BB_ERR_ARG; }
+    if (crs_view(crs).ctx != ctx) { set_error("%s: the key lives on another context", fn); return BB_ERR_ARG; }
+    BB_TRY(check_witness(fn, ctx, R, input, n_inputs, aux, n_aux, on_device, true));
+    if (own > 7) { set_error("%s: own = %u: bits 0, 1, 2 are a, b, c", fn, own); return BB_ERR_ARG; }
+    if (own && !d_evals) { set_error("%s: own = %u without evaluation vectors", fn, own); return BB_ERR_ARG; }
+    for (int i = 0; i < 3; i++)
+        if ((own >> i & 1) && (!d_evals[i] || !aligned16(d_evals[i]))) {
+            set_error("%s: evaluation vector %c is %s", fn, "abc"[i], d_evals[i] ? "not 16-byte aligned" : "null");
+            return BB_ERR_ARG;
+        }
     BB_CUDA(cudaSetDevice(ctx->device));
-    NvtxRange nvtx("prove_r1cs (upload, eval)");
-    cudaStream_t st = ctx->main_stream;
-    const size_t n = R->n;
-    StageTimer tm(ctx, st);
-    tm.mark("r1cs.begin");
-    DevBuf up[2], d_abc;
-    const Fr *d_in, *d_aux;
-    BB_TRY(stage_witness(ctx, st, input, n_inputs, aux, n_aux, on_device, up, &d_in, &d_aux));
-    // the prover copies the assignments on a stream of its own: the upload must be complete before it is called
-    // (the evaluation queued below need not be -- the witness MSMs do not wait for it)
-    if (!on_device) BB_CUDA(cudaStreamSynchronize(st));
-    tm.mark("r1cs.upload");
-    BB_TRY(d_abc.alloc(ctx, 3 * n * 32));
-    Fr* oa = d_abc.as<Fr>();
-    BB_TRY(r1cs_eval_queue(ctx, st, R, d_in, d_aux, oa, oa + n, oa + 2 * n));
-    tm.mark("r1cs.eval");
-    // create_proof from here on (prover.rs:217-360): the H pipeline reads a, b, c on the same stream, after the evaluation
-    bb_witness w{};
-    w.a = oa; w.b = oa + n; w.c = oa + 2 * n; w.n_constraints = n;
-    w.input_assignment = d_in; w.n_inputs = n_inputs;
-    w.aux_assignment = d_aux; w.n_aux = n_aux;
-    w.a_aux_density = R->a_aux_density.data();
-    w.b_input_density = R->b_input_density.data();
-    w.b_aux_density = R->b_aux_density.data();
-    w.on_device = 1;
-    const int rc = bb_groth16_prove(ctx, crs, &w, r, s, proof);
-    if (cudaStreamSynchronize(st) == cudaSuccess) tm.report(R->nnz[0] + R->nnz[1] + R->nnz[2]);
-    return rc;
+    NvtxRange nvtx("prove_r1cs_begin");
+    const bb_witness w = r1cs_witness(R, input, aux, on_device);
+    R1csStart start = d_evals ? R1csStart{true, {}, {}, 0} : r1cs_replicated(ctx, R);
+    if (own) {
+        size_t m;
+        uint32_t log_m;
+        BB_TRY(domain_size(R->n, &m, &log_m));
+        start.head = [=](cudaStream_t st, const Fr* d_in, const Fr* d_aux, Fr* tmp, StageTimer& tm) -> int {
+            for (int i = 0; i < 3; i++)
+                if (own >> i & 1) BB_TRY(r1cs_owner_queue(ctx, st, R, i, d_in, d_aux, (Fr*)d_evals[i], m, log_m, tmp, tm));
+            return BB_OK;
+        };
+    }
+    return prove_begin_r1cs(ctx, crs, &w, start, out);
 }
 
 // bb_groth16_prove_batch with the evaluation as its fill: each sub-batch uploads its witnesses once and evaluates every
@@ -437,6 +505,28 @@ int bb_groth16_prove_r1cs_batch(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* R
         return BB_OK;
     };
     return prove_batch_impl(ctx, crs, ws.data(), count, r, s, proofs, status, &fill);
+}
+
+int bb_diag_r1cs_owner_stage(bb_ctx* ctx, const bb_r1cs* R, const void* input, size_t n_inputs, const void* aux, size_t n_aux,
+                             int on_device, int poly, void* d_out) {
+    if (!ctx || !R || !d_out || poly < 0 || poly > 2) { set_error("bb_diag_r1cs_owner_stage: bad argument"); return BB_ERR_ARG; }
+    BB_TRY(check_witness("bb_diag_r1cs_owner_stage", ctx, R, input, n_inputs, aux, n_aux, on_device, aligned16(d_out)));
+    BB_CUDA(cudaSetDevice(ctx->device));
+    size_t m;
+    uint32_t log_m;
+    BB_TRY(domain_size(R->n, &m, &log_m));
+    cudaStream_t st = ctx->main_stream;
+    StageTimer tm(ctx, st);
+    tm.mark("r1cs_owner.begin");
+    DevBuf up[2], tmp;
+    const Fr *d_in, *d_aux;
+    BB_TRY(stage_witness(ctx, st, input, n_inputs, aux, n_aux, on_device, up, &d_in, &d_aux));
+    tm.mark("r1cs_owner.upload", 0);
+    BB_TRY(tmp.alloc(ctx, m * 32));
+    BB_TRY(r1cs_owner_queue(ctx, st, R, poly, d_in, d_aux, (Fr*)d_out, m, log_m, tmp.as<Fr>(), tm));
+    BB_CUDA(cudaStreamSynchronize(st));
+    tm.report(0);
+    return BB_OK;
 }
 
 int bb_r1cs_check(bb_ctx* ctx, const bb_r1cs* R, const void* input, size_t n_inputs, const void* aux, size_t n_aux, int on_device,

@@ -160,12 +160,60 @@ def create_proof_sharded(assignment, params, full_vk_params, r, s, device_ptrs=N
     the m evaluations; every rank then runs the last transform (a b - c, / Z, icoset_fft) itself.  The longest
     chain drops from seven transforms to three, and a rank uploads only the polynomials it owns.  The seven
     witness MSMs are queued first and run underneath."""
+    import bellman_b200 as bb
+
+    def start(bufs, own, lap):
+        n = assignment.a.shape[0]
+        for i, name in enumerate(("a", "b", "c")):
+            if own >> i & 1:
+                if device_ptrs is not None:
+                    bb.h_coset_evals_async(params.worker, device_ptrs[name], n, bufs[i].data_ptr(), on_device=True)
+                else:
+                    bb.h_coset_evals_async(params.worker, getattr(assignment, name), n, bufs[i].data_ptr())
+        lap("h_stage1_launch")
+        state = bb.prove_begin(assignment, params, device_ptrs)
+        lap("queue_witness_msms")
+        return state
+
+    return _prove_collective(lambda: assignment.a.shape[0], start, lambda: bb.prove_partials(assignment, params, device_ptrs),
+                             params, full_vk_params, r, s, group, split_h)
+
+
+def create_proof_r1cs_sharded(r1cs, params, full_vk_params, input_assignment, aux_assignment, r, s, device_ptrs=None, group=None,
+                              split_h=True):
+    """create_proof_sharded from the witness alone (bb_groth16_prove_r1cs_begin on every rank's key shard): the same
+    collective -- the h_owner split, every rank in every broadcast, one all-gather of partial sums, status and error text,
+    finalize on rank 0 -- but no rank evaluates a, b, c on the host or uploads them.  With split_h, rank h_owner(i)
+    evaluates matrix i alone straight into the buffer it broadcasts and transforms it there, launched before its witness
+    MSMs are queued; otherwise (or with one rank) every rank runs the whole H pipeline from its own copy of the witness.
+    Witness arguments as r1cs.create_proof_r1cs's.  Returns the 192 proof bytes on rank 0, None elsewhere."""
+    import bellman_b200 as bb
+    from . import r1cs as RC
+
+    def begin(own=0, evals=None):
+        return RC.prove_r1cs_begin(r1cs, params, input_assignment, aux_assignment, own, evals, device_ptrs)
+
+    def start(bufs, own, lap):
+        state = begin(own, [b.data_ptr() for b in bufs])      # the owner stage launched, then the witness MSMs queued
+        lap("r1cs_begin")
+        return state
+
+    return _prove_collective(lambda: r1cs.n_constraints, start, lambda: bb.prove_end(begin()),
+                             params, full_vk_params, r, s, group, split_h)
+
+
+def _prove_collective(n_constraints, start, partials, params, full_vk_params, r, s, group, split_h):
+    """The collective of one sharded proof.  A rank starts its proof one of two ways:
+    start(bufs, own, lap) -> the bb_prove state: polynomial i's coset evaluations launched into bufs[i] for every bit i
+    of `own` (the polynomials this rank owns), then the witness MSMs queued (lap(name) records a host phase);
+    partials() -> the 960 bytes of the whole proof on this rank (replicated H pipeline).
+    n_constraints() -> the rows of a, b, c."""
     import torch
     import torch.distributed as dist
 
     import threading
 
-    from . import BackendError, _ERRORS, finalize, finalize_static, h_coset_evals_async, h_coset_evals_wait, prove_begin, prove_end, prove_partials
+    from . import BackendError, _ERRORS, finalize, finalize_static, h_coset_evals_wait, prove_end
 
     rank, world = dist.get_rank(group), dist.get_world_size(group)
     backend = dist.get_backend(group)
@@ -183,8 +231,11 @@ def create_proof_sharded(assignment, params, full_vk_params, r, s, device_ptrs=N
         worker_thread = threading.Thread(target=_static)
         worker_thread.start()
     import time
-    t_ = time.perf_counter()
+    t_ = [time.perf_counter()]
     status, blob, msg = 0, bytes(PARTIALS_BYTES), ""
+
+    def lap(name):
+        t_[0] = _mark(name, t_[0])
 
     def code_of(e):
         return next((code for code, cls in _ERRORS.items() if isinstance(e, cls)), 17 if isinstance(e, BackendError) else 255)
@@ -198,10 +249,9 @@ def create_proof_sharded(assignment, params, full_vk_params, r, s, device_ptrs=N
         #    them keeps the critical chain first and the MSMs queued under it.
         # A failure is carried to the all-gather; the broadcasts are entered by every rank whatever happened
         # (nobody may skip a collective).
-        state, bufs, n = None, None, 0
-        launched = False
+        state, bufs = None, None
         try:
-            n = assignment.a.shape[0]
+            n = n_constraints()
             m = 1
             while m < n:
                 m *= 2
@@ -209,53 +259,41 @@ def create_proof_sharded(assignment, params, full_vk_params, r, s, device_ptrs=N
             if key not in _EVAL_BUFFERS:
                 _EVAL_BUFFERS[key] = [torch.empty((m, 4), dtype=torch.int64, device=device) for _ in range(3)]
             bufs = _EVAL_BUFFERS[key]
-            launched = True
-            for i, name in enumerate(("a", "b", "c")):
-                if h_owner(i, world) == rank:
-                    if device_ptrs is not None:
-                        h_coset_evals_async(params.worker, device_ptrs[name], n, bufs[i].data_ptr(), on_device=True)
-                    else:
-                        h_coset_evals_async(params.worker, getattr(assignment, name), n, bufs[i].data_ptr())
+            own = sum(1 << i for i in range(3) if h_owner(i, world) == rank)
+            state = start(bufs, own, lap)
         except Exception as e:
             msg, status = str(e), code_of(e)
-        t_ = _mark("h_stage1_launch", t_)
-        if status == 0:
-            try:
-                state = prove_begin(assignment, params, device_ptrs)
-            except Exception as e:
-                msg, status = str(e), code_of(e)
-        t_ = _mark("queue_witness_msms", t_)
-        if launched:
+        if bufs is not None:
             try:
                 h_coset_evals_wait(params.worker)
             except Exception as e:
                 if status == 0:
                     msg, status = str(e), code_of(e)
-        if bufs is None:                                 # the buffers could not even be made: take part with scratch ones
+        else:                                            # the buffers could not even be made: take part with scratch ones
             bufs = [torch.empty((1, 4), dtype=torch.int64, device=device) for _ in range(3)]
-        t_ = _mark("h_stage1_wait", t_)
+        lap("h_stage1_wait")
         pending = [dist.broadcast(bufs[i], src=h_owner(i, world), group=group, async_op=True) for i in range(3)]
         for p in pending:
             p.wait()
         if backend == "nccl":
             torch.cuda.current_stream().synchronize()
-        t_ = _mark("broadcast_wait", t_)
+        lap("broadcast_wait")
         if state is not None:
             try:
                 if status == 0:
                     blob = prove_end(state, [b.data_ptr() for b in bufs])
                 else:
-                    prove_end(state, None)               # drain and free what prove_begin queued
+                    prove_end(state, None)               # drain and free what the start queued
             except Exception as e:
                 if status == 0:
                     msg, status = str(e), code_of(e)
-        t_ = _mark("h_final_and_msm_waits", t_)
+        lap("h_final_and_msm_waits")
     else:
         try:
-            blob = prove_partials(assignment, params, device_ptrs)
+            blob = partials()
         except Exception as e:                           # whatever it is, the other ranks must not be left in the all-gather
             msg, status = str(e), code_of(e)
-        t_ = _mark("prove_partials", t_)
+        lap("prove_partials")
     # one collective: partial sums, status and (on failure) the failing rank's own message
     text = msg.encode("utf-8", "replace")[:MSG_BYTES].ljust(MSG_BYTES, b"\0")
     mine = torch.frombuffer(bytearray(blob + bytes([status]) + text), dtype=torch.uint8).to(device)
@@ -263,7 +301,7 @@ def create_proof_sharded(assignment, params, full_vk_params, r, s, device_ptrs=N
     dist.all_gather(out, mine, group=group)
     gathered = bytes(torch.stack(out).cpu().numpy().tobytes())       # one device->host copy for all ranks' blobs
     gathered = [gathered[i * len(mine):(i + 1) * len(mine)] for i in range(world)]
-    t_ = _mark("all_gather", t_)
+    lap("all_gather")
     if worker_thread is not None:
         worker_thread.join()
     for rk, g in enumerate(gathered):
@@ -273,6 +311,6 @@ def create_proof_sharded(assignment, params, full_vk_params, r, s, device_ptrs=N
             raise _ERRORS.get(code, BackendError)(f"rank {rk} failed with status {code}" + (f": {what}" if what else ""))
     if rank == 0:
         proof = finalize(full_vk_params, [g[:PARTIALS_BYTES] for g in gathered], r, s, static=ahead.get("static"))
-        _mark("finalize", t_)
+        lap("finalize")
         return proof
     return None

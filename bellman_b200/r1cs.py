@@ -222,6 +222,27 @@ def create_proof_r1cs(r1cs, params, input_assignment, aux_assignment, r, s, devi
     return bytes(proof)
 
 
+class _ProveState(C.c_void_p):
+    """a bb_prove handle that keeps the host witness it was begun from alive until prove_end"""
+
+
+def prove_r1cs_begin(r1cs, params, input_assignment, aux_assignment, own=0, evals=None, device_ptrs=None):
+    """bb_groth16_prove_r1cs_begin on any key, sharded or not -> the state bellman_b200.prove_end(state, evals) ends.
+    evals = three device addresses (m Fr each; split mode): the polynomials whose bit is set in `own` (1 = a, 2 = b, 4 = c)
+    are evaluated from the witness straight into theirs and taken through ifft + coset_fft, ahead of the witness MSMs;
+    h_coset_evals_wait(worker) waits for them, and prove_end takes the three vectors once every rank's are there.
+    evals = None (replicated mode, own = 0): the whole H pipeline runs here and prove_end takes no vectors.  Witness
+    arguments as create_proof_r1cs's."""
+    if device_ptrs is not None:
+        input_assignment, aux_assignment = device_ptrs["inputs"], device_ptrs["aux"]
+    src, keep = r1cs._witness_args(input_assignment, aux_assignment, device_ptrs is not None)
+    d_evals = None if evals is None else (C.c_void_p * 3)(*(_addr(p) for p in evals))
+    state = _ProveState()
+    _check(load_library().bb_groth16_prove_r1cs_begin(params.worker._h, params._h, r1cs._h, *src, C.c_uint(own), d_evals, C.byref(state)))
+    state.keep = keep
+    return state
+
+
 def create_random_proof_r1cs(r1cs, params, input_assignment, aux_assignment, rng=None, device_ptrs=None):
     """create_random_proof (prover.rs:164-179) from the witness alone: r, s <- Fr::random, then create_proof_r1cs"""
     import secrets

@@ -89,8 +89,8 @@ void bb_ctx_destroy(bb_ctx* ctx);
  *   params_read_chunk  bb_params_read / bb_vk_read from host memory: staging bytes per chunk (default 64 MiB; rounded
  *                      down to whole points, at least one point)
  *   ntt_tile_log, ntt_col_bits   shape of the NTT tiles
- *   profile            1 = CUDA-event timing of the MSM stages, and of the verify.*, decode.*, r1cs.*, r1cs_check.*,
- *                      params.* and generate.* stages (bb_profile_read)
+ *   profile            1 = CUDA-event timing of the MSM stages, and of the verify.*, decode.*, r1cs.*, r1cs_owner.*,
+ *                      r1cs_check.*, h_coset_evals, params.* and generate.* stages (bb_profile_read)
  *   msm_acc_variant, msm_affine_tma, msm_reduce_2d, ntt_radix8   retired: accepted for compatibility, no effect */
 int bb_ctx_set_option(bb_ctx* ctx, const char* key, long value);
 int bb_ctx_synchronize(bb_ctx* ctx);
@@ -240,7 +240,8 @@ int bb_groth16_prove_begin(bb_ctx* ctx, const bb_crs* crs, const bb_witness* w, 
 int bb_groth16_prove_end(bb_prove* state, const void* d_evals_a, const void* d_evals_b, const void* d_evals_c,
                          uint8_t partials[BB_PARTIALS_BYTES]);
 /* d_out[0..m) = coset_fft(ifft(from_coeffs(poly))) for one polynomial of n_constraints Fr (Montgomery; host
- * memory, or device memory with on_device != 0); m = next power of two >= n_constraints.  Blocking. */
+ * memory, or device memory with on_device != 0); m = next power of two >= n_constraints.  Blocking.  Profile mode: the
+ * stage h_coset_evals (copy, padding, transforms; units n_constraints). */
 int bb_h_coset_evals(bb_ctx* ctx, const void* poly, size_t n_constraints, int on_device, void* d_out);
 /* The same without blocking: _async queues the copy and the two transforms on the context's high-priority stream
  * and returns at once (poly and d_out must stay valid); _wait blocks until every evaluation queued so far is
@@ -333,6 +334,32 @@ int bb_r1cs_eval(bb_ctx* ctx, const bb_r1cs* r1cs, const void* input, size_t n_i
  * device work; then exactly bb_groth16_prove's errors and their precedence. */
 int bb_groth16_prove_r1cs(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* r1cs, const void* input, size_t n_inputs,
                           const void* aux, size_t n_aux, int on_device, const uint8_t r[32], const uint8_t s[32], uint8_t proof[192]);
+/* bb_groth16_prove_begin from the witness alone, on any key -- shard k of count, 1 of 1 included -- for multi-GPU provers
+ * that split the H pipeline by polynomial.  The state is ended by bb_groth16_prove_end.
+ * Upload: the witness crosses the bus once, into the state, on its upload stream (on_device != 0: the caller's arrays are
+ * read in place); the evaluation and the witness MSMs read that copy.  Host->device bytes are bb_groth16_prove_begin's for
+ * the same witness; no a, b or c bytes cross the bus.
+ * Split mode (d_evals != NULL): for every polynomial i with bit 1 << i of `own` set (0 = a, 1 = b, 2 = c), matrix i alone
+ * is evaluated straight into d_evals[i] (m Fr, device, 16-byte aligned; zeros from n_constraints to m) and taken through
+ * ifft + coset_fft there (prover.rs:225-230): what bb_h_coset_evals gives for that polynomial.  These are queued FIRST, on
+ * the context's high-priority main stream behind the upload; then this shard's seven witness MSMs are queued and the call
+ * returns.  own = 0 launches no evaluation kernel.  bb_h_coset_evals_wait(ctx) waits for the owned vectors; after the
+ * broadcast, bb_groth16_prove_end(state, a, b, c, partials) runs the last transform, the h MSM and the waits.
+ * Replicated mode (d_evals == NULL, own = 0): the three matrices are evaluated into the H pipeline's own rows and the whole
+ * H pipeline and the h MSM are queued first, then the witness MSMs (bb_groth16_prove_r1cs's order);
+ * bb_groth16_prove_end(state, NULL, NULL, NULL, partials) ends it.
+ * Argument errors, BB_ERR_ARG before any device work: a NULL ctx, crs, r1cs or out; a key or constraint system of another
+ * context; bb_r1cs_eval's witness checks; own > 7; own != 0 without d_evals; an owned d_evals[i] NULL or misaligned.
+ * Ending a split state without the three vectors, or a replicated state with them, is BB_ERR_ARG and frees the state.  On
+ * any failure *out is NULL and nothing stays queued.
+ * Results: bb_groth16_prove_end reports the MSM errors as for a bb_groth16_prove_begin state (the density assert, delta =
+ * identity, then the reference's wait order); the partial sums of all shards, through bb_groth16_finalize, are
+ * bb_groth16_prove_r1cs's bytes on the unsharded key.  An unsatisfied witness proves, as in the reference.  Profile mode:
+ * the owner stage's stages r1cs_owner.upload (main stream waiting for the witness), r1cs_owner.eval, r1cs_owner.transforms
+ * (bb_profile_read; units: 0, the owned matrix's terms, m; one record per owned polynomial), recorded when
+ * bb_groth16_prove_end returns. */
+int bb_groth16_prove_r1cs_begin(bb_ctx* ctx, const bb_crs* crs, const bb_r1cs* r1cs, const void* input, size_t n_inputs,
+                                const void* aux, size_t n_aux, int on_device, unsigned own, void* const d_evals[3], bb_prove** out);
 /* bb_groth16_prove_batch from witnesses alone: inputs = count x n_inputs Fr and aux = count x n_aux Fr, row-major (host, or
  * device memory with on_device != 0).  status[i] and proof i are bb_groth16_prove_r1cs's for item i alone.  Argument errors
  * as bb_r1cs_eval's and bb_groth16_prove_batch's, before any device work. */

@@ -84,6 +84,12 @@ int bb_diag_points_decompress(bb_ctx* ctx, int group, const void* bytes, size_t 
  * that vector: all of them on a single GPU); which 5 = alpha_g1, beta_g1, delta_g1 (96 B each) then beta_g2, delta_g2
  * (192 B each) */
 int bb_diag_crs_download(const bb_crs* crs, int which, void* out);
+/* The owner stage of bb_groth16_prove_r1cs_begin for polynomial `poly` (0 = a, 1 = b, 2 = c) alone, with no MSM in flight:
+ * the witness uploaded (on_device = 0) or read in place, matrix poly evaluated into d_out (m Fr, device, 16-byte aligned),
+ * zeros to m, ifft + coset_fft there; on the main stream, blocking.  Profile mode records the stages r1cs_owner.upload,
+ * r1cs_owner.eval (units: the matrix's terms) and r1cs_owner.transforms (units: m), as the split mode does. */
+int bb_diag_r1cs_owner_stage(bb_ctx* ctx, const bb_r1cs* r1cs, const void* input, size_t n_inputs, const void* aux, size_t n_aux,
+                             int on_device, int poly, void* d_out);
 /* bytes of device memory the context has handed out and not yet taken back (its cache of free blocks excluded) */
 uint64_t bb_diag_ctx_live_bytes(const bb_ctx* ctx);
 

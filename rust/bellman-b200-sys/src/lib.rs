@@ -3,7 +3,7 @@
 //! (x | y, Montgomery limbs), G2 affine = 192 bytes (x.c0 | x.c1 | y.c0 | y.c1), identity = all zero.
 #![allow(non_camel_case_types)]
 
-use std::os::raw::{c_char, c_int, c_long, c_void};
+use std::os::raw::{c_char, c_int, c_long, c_uint, c_void};
 
 #[repr(C)] pub struct bb_ctx { _private: [u8; 0] }
 #[repr(C)] pub struct bb_bases { _private: [u8; 0] }
@@ -213,6 +213,9 @@ extern "C" {
                         n_aux: usize, in_on_device: c_int, a: *mut c_void, b: *mut c_void, c: *mut c_void, out_on_device: c_int) -> c_int;
     pub fn bb_groth16_prove_r1cs(ctx: *mut bb_ctx, crs: *const bb_crs, r1cs: *const bb_r1cs, input: *const c_void, n_inputs: usize,
                                  aux: *const c_void, n_aux: usize, on_device: c_int, r: *const u8, s: *const u8, proof: *mut u8) -> c_int;
+    pub fn bb_groth16_prove_r1cs_begin(ctx: *mut bb_ctx, crs: *const bb_crs, r1cs: *const bb_r1cs, input: *const c_void, n_inputs: usize,
+                                       aux: *const c_void, n_aux: usize, on_device: c_int, own: c_uint, d_evals: *const *mut c_void,
+                                       out: *mut *mut bb_prove) -> c_int;
     pub fn bb_groth16_prove_r1cs_batch(ctx: *mut bb_ctx, crs: *const bb_crs, r1cs: *const bb_r1cs, inputs: *const c_void,
                                        n_inputs: usize, aux: *const c_void, n_aux: usize, count: usize, on_device: c_int,
                                        r: *const u8, s: *const u8, proofs: *mut u8, status: *mut c_int) -> c_int;

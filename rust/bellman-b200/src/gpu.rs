@@ -386,6 +386,54 @@ pub fn create_proof_r1cs_b200<C: Circuit<Scalar>>(circuit: C, r1cs: &GpuR1cs, cr
     Proof::read(&bytes[..]).map_err(Into::into)
 }
 
+/// One rank's part of a proof from the witness on a sharded key (bb_groth16_prove_r1cs_begin): `begin` uploads the witness
+/// once and, for every polynomial whose bit is set in `own` (1 = a, 2 = b, 4 = c), evaluates its matrix straight into
+/// `d_evals[i]` (m Fr, device) and takes it through ifft + coset_fft, ahead of this shard's seven witness MSMs.  After
+/// `bb_h_coset_evals_wait` and the broadcast of the owners' vectors, `end` runs the last transform, the h MSM and the
+/// waits and returns the 960-byte partial sums for `bb_groth16_finalize`.  `d_evals = None` (own = 0) runs the whole H
+/// pipeline on this rank; `end(None)` finishes it.
+pub struct GpuR1csProof { handle: *mut bb_prove }
+unsafe impl Send for GpuR1csProof {}
+
+impl GpuR1cs {
+    /// # Safety
+    /// `input_assignment` and `aux_assignment` must stay alive and unchanged until the returned state is ended or
+    /// dropped: the library reads them asynchronously.  Every `d_evals[i]` with bit `1 << i` set in `own`, and all three
+    /// given to `end`, must be device allocations of m Fr (m = the next power of two >= the constraints), 16-byte
+    /// aligned, of this worker's device, not read or written by anything else until `bb_h_coset_evals_wait` returns (an
+    /// owned one) or `end` returns; the library writes the owned ones and overwrites the first one given to `end`.
+    pub unsafe fn begin(&self, crs: &GpuParameters, input_assignment: &[Scalar], aux_assignment: &[Scalar], own: u32,
+                 d_evals: Option<[*mut c_void; 3]>) -> Result<GpuR1csProof, SynthesisError> {
+        let mut handle = ptr::null_mut();
+        let evals = d_evals.as_ref().map_or(ptr::null(), |e| e.as_ptr());
+        status(unsafe {
+            bb_groth16_prove_r1cs_begin(crs.ctx, crs.handle, self.handle, input_assignment.as_ptr() as _, input_assignment.len(),
+                                        aux_assignment.as_ptr() as _, aux_assignment.len(), 0, own, evals, &mut handle)
+        })?;
+        Ok(GpuR1csProof { handle })
+    }
+}
+
+impl GpuR1csProof {
+    /// # Safety
+    /// The three vectors must be valid as `GpuR1cs::begin` requires.
+    pub unsafe fn end(mut self, d_evals: Option<[*const c_void; 3]>) -> Result<[u8; 960], SynthesisError> {
+        let mut partials = [0u8; 960];
+        let [a, b, c] = d_evals.unwrap_or([ptr::null(); 3]);
+        let handle = std::mem::replace(&mut self.handle, ptr::null_mut());
+        status(unsafe { bb_groth16_prove_end(handle, a, b, c, partials.as_mut_ptr()) })?;     // frees the state, also on an error
+        Ok(partials)
+    }
+}
+impl Drop for GpuR1csProof {
+    fn drop(&mut self) {                                       // never ended: drain and free (with vectors or without, one is refused)
+        if !self.handle.is_null() {
+            let mut partials = [0u8; 960];
+            unsafe { bb_groth16_prove_end(self.handle, ptr::null(), ptr::null(), ptr::null(), partials.as_mut_ptr()) };
+        }
+    }
+}
+
 /// Drop-in for the body of `groth16::create_proof` after synthesis (groth16/src/prover.rs:217-360).
 /// `Scalar` is `[u64; 4]` in Montgomery form (R = 2^256), which is BB_FORM_MONTGOMERY byte for byte; the
 /// cast below is version-pinned (`bls12_381 = "=0.8.0"`) because `#[repr(transparent)]` is not promised.
