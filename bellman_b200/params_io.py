@@ -19,7 +19,9 @@ limbs, identity = all-zero) and applies the reference's acceptance rules:
   (lib.rs:158-183 has no unchecked mode), for the five vectors when `checked=True`
   (lib.rs:294-298,328-332).  This is curve arithmetic, so it runs on the device
   (`bb_points_validate`): pass the `Worker` to use, or one is created on device 0 -- without a CUDA
-  device the call fails, there is no CPU fallback.
+  device the call fails, there is no CPU fallback.  Zero coordinates without the infinity flag are
+  the point (0, 0), off the curve, and fail this check; unchecked, they load as the all-zero
+  identity (DESIGN.md section 7).
 
 `read_parameters_device` / `read_verifying_key_device` read the same files on the device
 (`bb_params_read` / `bb_vk_read`): the bytes are decoded and checked there, straight into a
@@ -106,6 +108,12 @@ def _read_points(buf, off, count, g2, what, allow_infinity, validate):
     if count:
         out[inf] = 0
     if validate is not None and count:
+        # zeros without the infinity flag are the point (0, 0), which is not on the curve; the ABI's all-zero identity
+        # cannot stand for it, so it is rejected here, after the points before it are checked
+        zero = np.flatnonzero(~out.any(axis=1) & ~inf)
+        if zero.size:
+            validate(g2, out[:zero[0]], what)
+            raise InvalidData(f"invalid {name}: {what}[{int(zero[0])}] is not on the curve")
         validate(g2, out, what)
     return out, end
 
